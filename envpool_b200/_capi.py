@@ -38,7 +38,7 @@ ABI_SYMBOLS = [
     "epb_exchange_attach_ipc", "epb_step_exchange_device", "epb_exchange_wait",
     "epb_exchange_status", "epb_exchange_slice_bytes", "epb_exchange_depth",
     "epb_step_many_timed", "epb_step_exchange_many_device", "epb_fp64_peak_gflops",
-    "epb_hc_model", "epb_exchange_trace",
+    "epb_hc_model", "epb_hc_pair_rows", "epb_exchange_trace",
 ]
 IPC_HANDLE_BYTES = 64
 
@@ -126,6 +126,7 @@ def load_library() -> ctypes.CDLL:
     L.epb_exchange_trace.argtypes = [vp, vp, ctypes.c_int64]
     L.epb_hc_model.restype = ctypes.c_int64
     L.epb_hc_model.argtypes = [vp, ctypes.c_int64]
+    L.epb_hc_pair_rows.argtypes = [vp, ci]
     _lib = L
     return L
 
@@ -474,6 +475,11 @@ class CPool:
     @property
     def bytes_per_env_step(self) -> int:
         return self.lib.epb_bytes_per_env_step(self.h)
+
+    def hc_pair_rows(self, n: Optional[int] = None) -> int:
+        """HalfCheetah's two-lane kernel: constraint rows per lane held in shared memory for a
+        launch of n batch rows (default num_envs); 0 for any other kernel or env."""
+        return self.lib.epb_hc_pair_rows(self.h, self.n if n is None else n)
 
     def state_layout(self) -> Dict[str, int]:
         out = (ctypes.c_int64 * 12)()

@@ -1683,6 +1683,11 @@ int epb_fp64_peak_gflops(int device, double* gflops_out) {
 }
 
 int64_t epb_hc_model(void* dst, int64_t cap) { return mjc_model_blob(dst, cap); }
+int epb_hc_pair_rows(const epb_pool* p, int n) {
+  if (!p || !p->mjc || n <= 0 || n > p->N) return 0;
+  DeviceGuard guard(p->cfg.device);  // the SM count is read from the pool's device
+  return guard.status == cudaSuccess ? mjc_pair_rows(p->mjc, n) : 0;
+}
 int64_t epb_launch_count(const epb_pool* p) { return p ? p->launches : 0; }
 int epb_bytes_per_env_step(const epb_pool* p) { return p ? p->bytes_per_step : 0; }
 

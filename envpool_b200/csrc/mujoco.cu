@@ -1075,6 +1075,8 @@ static int pair_rows_in_smem(int n) {
   return ks < kPairKsMin ? kPairKsMin : ks;
 }
 
+int mjc_pair_rows(const MjcPool* m, int n) { return m->variant == 0 ? pair_rows_in_smem(n) : 0; }
+
 static void launch_pair(MjcPool* m, const StateView& sv, const OutView& ov, const double* d_action,
                         const int32_t* d_env_ids, int n, int force_reset, int T,
                         cudaStream_t stream) {
