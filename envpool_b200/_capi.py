@@ -478,7 +478,8 @@ class CPool:
 
     def hc_pair_rows(self, n: Optional[int] = None) -> int:
         """HalfCheetah's two-lane kernel: constraint rows per lane held in shared memory for a
-        launch of n batch rows (default num_envs); 0 for any other kernel or env."""
+        launch of n batch rows (default num_envs); 0 for any other env or n outside
+        [1, num_envs]."""
         return self.lib.epb_hc_pair_rows(self.h, self.n if n is None else n)
 
     def state_layout(self) -> Dict[str, int]:

@@ -1,6 +1,6 @@
-// HalfCheetah model constants shared by the physics kernels (mujoco.cu, mujoco_thread.cuh,
-// mujoco_pair.cuh) and by the host-side emulation of the pair-lane kernel used in the CPU
-// tests.  Plain C++: no CUDA types.  What each field restates of
+// HalfCheetah model constants shared by the physics kernel (mujoco.cu, mujoco_pair.cuh) and
+// by the host-side emulation of the pair-lane kernel used in the CPU tests.  Plain C++: no
+// CUDA types.  What each field restates of
 // third_party/mujoco_gym_xml_patches/half_cheetah_envpool.xml is documented where it is
 // filled, compile_half_cheetah (mujoco.cu).
 #pragma once

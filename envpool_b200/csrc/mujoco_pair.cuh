@@ -1,4 +1,4 @@
-// HalfCheetah physics, TWO LANES PER ENV (the default kernel).
+// HalfCheetah physics, TWO LANES PER ENV.
 //
 // The cheetah's kinematic tree is torso | back leg | front leg, and every matrix of the
 // step -- M, H = M + J^T D J, M + h B -- is block-arrow over exactly that split (no
@@ -13,10 +13,10 @@
 //
 // Both lanes execute the SAME instruction stream (SIMT-friendly: no role divergence), each on
 // half the rows, half of the kinematic chain and 21 instead of 36 matrix entries; a warp
-// carries 16 envs.  Against the one-thread-per-env kernel (mujoco_thread.cuh) the dependent
-// chain of one mj_step is ~0.6x as long, nothing is indexed by a runtime leg id any more
-// (which had put H, fc and the solver vectors into local memory), and the constraint rows of
-// a lane live in shared memory (first `ks` rows; the rare rest in thread-local overflow).
+// carries 16 envs.  Against one thread per env, the dependent chain of one mj_step is ~0.6x
+// as long, nothing is indexed by a runtime leg id (which put H, fc and the solver vectors
+// into local memory there), and the constraint rows of a lane live in shared memory (first
+// `ks` rows; the rare rest in thread-local overflow).
 //
 // Dual build: with HCP_HOST defined this header compiles as plain C++ (two host threads play
 // the lane pair and meet at every exchange, tests/hc_pair_host/); the CPU test suite checks

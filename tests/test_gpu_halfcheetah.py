@@ -1,4 +1,4 @@
-"""GPU: HalfCheetah (default kernel: two lanes per env) against the CPU restatement of the same
+"""GPU: HalfCheetah (two lanes per env) against the CPU restatement of the same
 pipeline (oracle/mjc_oracle.c).  PARITY UNPINNED against MuJoCo 3.6.0 itself -- see the
 oracle's header and DESIGN.md.  Tolerances: the kernel and the oracle differ only in
 summation order / FMA contraction / libm (1e-16 relative per operation); one teacher-forced
@@ -6,10 +6,6 @@ env step (5 mj_steps, Newton solves included) must agree to 1e-9; free-running t
 are compared over a short horizon because contact dynamics amplify rounding noise (the
 reference's own precedent for MuJoCo: 5e-3 over <= 64 steps on arm64,
 mujoco_gym_align_test.py:42-43,93-94)."""
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
@@ -129,16 +125,3 @@ def test_python_api_halfcheetah(capi):
     np.testing.assert_allclose(info["reward_ctrl"], -0.1 * (a * a).sum(1), rtol=1e-12)
     assert env.spec.config.max_episode_steps == 1000
 
-
-@pytest.mark.parametrize("variant", ["thread", "warp"])
-def test_alternative_kernels(variant):
-    """The thread-per-env and warp-per-env kernels stay selectable (ENVPOOL_B200_HC_KERNEL, read
-    at pool creation): the reset and teacher-forced checks above, re-run in a subprocess with
-    the switch set, keep them honest."""
-    env = dict(os.environ, ENVPOOL_B200_HC_KERNEL=variant)
-    r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-q", "-x",
-                        "-p", "no:cacheprovider", "-k", "reset_draws or teacher_forced"],
-                       env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True,
-                       timeout=600)
-    assert r.returncode == 0, r.stdout[-3000:]
-    assert "2 passed" in r.stdout, r.stdout[-1000:]
