@@ -558,6 +558,10 @@ rollout_kernel(StateView sv, OutView ov, const typename Env::Act* __restrict__ a
             Mt rng(sv, eid, mt_idx);
             Env::reset(sv, s, &rng, so);
             mt_idx = rng.idx;
+            // a record produced and consumed at once: the counters keep counting records, so
+            // the refill below puts record i in slot i % rec_q, as the state layout promises
+            ++rp;
+            ++rc;
           }
         }
         flags = (cur << 1) | done;

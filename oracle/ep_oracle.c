@@ -838,6 +838,9 @@ void epo_get_state(const epo_pool* p, int eid, double* s5, int* done, int* cur) 
   *done = e->done;
   *cur = e->current_step;
 }
+void epo_get_states(const epo_pool* p, double* s5) {
+  for (int e = 0; e < p->num_envs; ++e) memcpy(s5 + (size_t)e * 5, p->envs[e].s, sizeof(double) * 5);
+}
 void epo_set_state(epo_pool* p, int eid, const double* s5, int done, int cur) {
   epo_env* e = &p->envs[eid];
   for (int k = 0; k < 5; ++k) e->s[k] = s5[k];

@@ -62,6 +62,8 @@ int epo_action_row_elems(const epo_pool* p);
  * one) without touching its RNG */
 void epo_get_state(const epo_pool* p, int eid, double* s5, int* done, int* cur);
 void epo_set_state(epo_pool* p, int eid, const double* s5, int done, int cur);
+/* s[0..4] of every env at once: s5 is [num_envs][5] */
+void epo_get_states(const epo_pool* p, double* s5);
 /* HalfCheetah teacher forcing: s27 = qpos[9] qvel[9] qacc_warmstart[9] */
 void epo_mjc_set(epo_pool* p, int eid, const double* s27, int done, int cur);
 void epo_mjc_get(const epo_pool* p, int eid, double* s27);

@@ -56,6 +56,7 @@ def lib():
         L.epo_action_row_elems.argtypes = [vp]
         L.epo_get_state.argtypes = [vp, ci, vp, vp, vp]
         L.epo_set_state.argtypes = [vp, ci, vp, ci, ci]
+        L.epo_get_states.argtypes = [vp, vp]
         L.epo_mjc_set.argtypes = [vp, ci, vp, ci, ci]
         L.epo_mjc_get.argtypes = [vp, ci, vp]
         L.epo_debug_draw.restype = ctypes.c_uint32
@@ -151,6 +152,12 @@ class OraclePool:
         d, c = ctypes.c_int(), ctypes.c_int()
         lib().epo_get_state(self.h, eid, buf, ctypes.byref(d), ctypes.byref(c))
         return list(buf), d.value, c.value
+
+    def states(self):
+        """[num_envs, 5] continuous state s[0..4] of every env."""
+        out = np.zeros((self.n, 5))
+        lib().epo_get_states(self.h, out.ctypes.data)
+        return out
 
     def mjc_set(self, eid, s27, done, cur):
         buf = np.ascontiguousarray(s27, dtype=np.float64)
