@@ -23,6 +23,7 @@ KINDS = {
     "CartPole": 0, "Pendulum": 1, "Acrobot": 2, "MountainCar": 3,
     "MountainCarContinuous": 4, "FrozenLake": 5, "Catch": 6, "Taxi": 7,
     "NChain": 8, "CliffWalking": 9, "Blackjack": 10, "HalfCheetah": 11,
+    "Game2048": 12,
 }
 DTYPES = {0: np.int32, 1: np.float32, 2: np.float64, 3: np.bool_}
 
@@ -38,7 +39,7 @@ ABI_SYMBOLS = [
     "epb_exchange_attach_ipc", "epb_step_exchange_device", "epb_exchange_wait",
     "epb_exchange_status", "epb_exchange_slice_bytes", "epb_exchange_depth",
     "epb_step_many_timed", "epb_step_exchange_many_device", "epb_fp64_peak_gflops",
-    "epb_hc_model", "epb_hc_pair_rows", "epb_exchange_trace",
+    "epb_hc_model", "epb_hc_pair_rows", "epb_exchange_trace", "epb_game2048_boards",
 ]
 IPC_HANDLE_BYTES = 64
 
@@ -127,6 +128,7 @@ def load_library() -> ctypes.CDLL:
     L.epb_hc_model.restype = ctypes.c_int64
     L.epb_hc_model.argtypes = [vp, ctypes.c_int64]
     L.epb_hc_pair_rows.argtypes = [vp, ci]
+    L.epb_game2048_boards.argtypes = [vp, vp, vp]
     _lib = L
     return L
 
@@ -481,6 +483,17 @@ class CPool:
         launch of n batch rows (default num_envs); 0 for any other env or n outside
         [1, num_envs]."""
         return self.lib.epb_hc_pair_rows(self.h, self.n if n is None else n)
+
+    def game2048_boards(self, initial=None, replay=None):
+        """Game2048's configured boards, before the first reset: `initial` is 16 tile exponents
+        (row-major), `replay` 32 boards of 16; None = not configured.  Cells outside [0, 26]
+        raise ValueError."""
+        ini = None if initial is None else np.ascontiguousarray(initial, dtype=np.int32).ravel()
+        rep = None if replay is None else np.ascontiguousarray(replay, dtype=np.int32).ravel()
+        if (ini is not None and ini.size != 16) or (rep is not None and rep.size != 512):
+            raise ValueError("Game2048 boards: 16 initial cells and 32 x 16 replay cells")
+        _check(self.lib.epb_game2048_boards(self.h, None if ini is None else ini.ctypes.data,
+                                            None if rep is None else rep.ctypes.data))
 
     def state_layout(self) -> Dict[str, int]:
         out = (ctypes.c_int64 * 12)()

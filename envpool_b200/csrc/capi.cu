@@ -77,6 +77,10 @@ struct Key {
   int64_t off;
 };
 
+// Game2048's configured boards (epb_game2048_boards): initial + 32 replay boards, 3 words each
+constexpr int kGame2048ConfigWords = 3 + 32 * 3;
+constexpr int kGame2048MaxCell = 26;
+
 static int dtype_size(int d) { return d == EPB_F64 ? 8 : d == EPB_BOOL ? 1 : 4; }
 
 // What a cached chain graph was captured for.
@@ -161,6 +165,7 @@ struct epb_pool {
   cudaEvent_t ev_mark = nullptr, ev_t0 = nullptr, ev_t1 = nullptr;
   int64_t launches = 0;
   int bytes_per_step = 0;
+  bool started = false;  // a step, reset or rollout has been launched
   // peer exchange (exchange.cuh):
   //   slot[D][world][x_slice] | data_flag[16] | ack_flag[16] | ctl | PeerView[D]
   char* x_base = nullptr;
@@ -261,6 +266,12 @@ int build_keys(epb_pool* p) {
       p->NI = 1;
       break;
     case EPB_BLACKJACK: add_key(p, "obs", EPB_I32, {3}); p->NI = 2; break;
+    case EPB_GAME2048:  // jumanji/game2048_env.h Game2048EnvFns::StateSpec
+      add_key(p, "obs:board", EPB_I32, {4, 4});
+      add_key(p, "obs:action_mask", EPB_BOOL, {4});
+      add_key(p, "info:highest_tile", EPB_I32, {});
+      p->NI = 3;
+      break;
     case EPB_HALF_CHEETAH:
       // mujoco/gym/half_cheetah.h:44-62
       add_key(p, "obs", EPB_F64, {17});
@@ -542,6 +553,7 @@ int launch_batch(epb_pool* p, const void* d_action, const int32_t* d_ids, int n,
                  const PeerView* peers = nullptr, int chain_k = -1, int32_t* wire = nullptr,
                  const void* next_action = nullptr) {
   p->d_last = d_slab;
+  p->started = true;
   if (p->kind == EPB_HALF_CHEETAH) {
     OutView hov = p->slab_view(d_slab);
     hov.wire = wire;
@@ -697,7 +709,11 @@ int epb_create(int kind, const epb_config* cfg, epb_pool** out) {
     return fail(EPB_ERR_INVALID, "unknown env kind");
   }
   int iopt = cfg->iopt;
-  if (iopt < 0) iopt = kind == EPB_FROZEN_LAKE ? 4 : kind == EPB_BLACKJACK ? 2 : 0;
+  if (iopt < 0) iopt = kind == EPB_FROZEN_LAKE ? 4 : kind == EPB_BLACKJACK ? 2 : kind == EPB_GAME2048 ? 1 : 0;
+  if (kind == EPB_GAME2048 && iopt > 1) {
+    delete p;
+    return fail(EPB_ERR_INVALID, "Game2048 iopt (add_random_cell) must be -1, 0 or 1");
+  }
   if (kind == EPB_FROZEN_LAKE && iopt != 4 && iopt != 8) {
     delete p;
     return fail(EPB_ERR_INVALID, "FrozenLake size must be 4 or 8");
@@ -722,7 +738,9 @@ int epb_create(int kind, const epb_config* cfg, epb_pool** out) {
   int64_t o_idx = o_flags + al(4 * N);
   int64_t o_ist = o_idx + al(4 * N);
   int64_t o_rst = o_ist + al(4 * N * (p->NI > 0 ? p->NI : 1));
-  int64_t o_mt = o_rst + al((int64_t)p->real_size * N * (p->NR > 0 ? p->NR : 1));
+  // Game2048 keeps its configured boards where real-valued envs keep rstate (jumanji.cu)
+  int64_t o_mt = o_rst + al(kind == EPB_GAME2048 ? 4 * kGame2048ConfigWords
+                                                 : (int64_t)p->real_size * N * (p->NR > 0 ? p->NR : 1));
   const bool has_rec = kind <= EPB_MOUNTAIN_CAR_CONTINUOUS;  // classic_control: record resets
   int rec_q = 16;  // records per env; ENVPOOL_B200_REC_Q = 4 | 8 | 16
   if (const char* rq = getenv("ENVPOOL_B200_REC_Q")) {
@@ -815,6 +833,9 @@ int epb_create(int kind, const epb_config* cfg, epb_pool** out) {
   } else if (kind <= EPB_BLACKJACK) {
     p->step_fn = toytext_step_fn(kind, iopt);
     p->rollout_fn = toytext_rollout_fn(kind, iopt);
+  } else if (kind == EPB_GAME2048) {
+    p->step_fn = jumanji_step_fn(kind);
+    p->rollout_fn = jumanji_rollout_fn(kind);
   }
 
   // seed on device
@@ -849,6 +870,7 @@ int epb_create(int kind, const epb_config* cfg, epb_pool** out) {
   for (const Key& k : p->keys) b += k.row_bytes;
   if (kind == EPB_FROZEN_LAKE || (kind == EPB_CLIFF_WALKING && iopt)) b += 16 + 8;
   if (kind == EPB_NCHAIN) b += 32 + 8;
+  if (kind == EPB_GAME2048) b += 3 * 16 + 8;  // 3 words per moving step (bernoulli 2, Lemire 1)
   if (kind == EPB_HALF_CHEETAH) b -= 2 * (32 - 27) * 8;  // 27 of the 32-double record are live
   p->bytes_per_step = b;
   *out = p;
@@ -1098,6 +1120,7 @@ int epb_rollout_device(epb_pool* p, const void* d_actions, int T, void* const* d
   ov.trunc = static_cast<uint8_t*>(d_cols[7]);
   for (size_t k = 8; k < p->keys.size(); ++k) ov.env[k - 8] = d_cols[k];
   ov.t_stride_rows = p->N;
+  p->started = true;
   if (p->kind == EPB_HALF_CHEETAH) {
     EPB_CUDA(mjc_launch_rollout(p->mjc, p->sv, ov, static_cast<const double*>(d_actions), T, s));
     ++p->launches;
@@ -1687,6 +1710,34 @@ int epb_hc_pair_rows(const epb_pool* p, int n) {
   if (!p || !p->mjc || n <= 0 || n > p->N) return 0;
   DeviceGuard guard(p->cfg.device);  // the SM count is read from the pool's device
   return guard.status == cudaSuccess ? mjc_pair_rows(p->mjc, n) : 0;
+}
+int epb_game2048_boards(epb_pool* p, const int32_t* initial16, const int32_t* replay512) {
+  if (!p) return fail(EPB_ERR_INVALID, "null pool");
+  if (p->kind != EPB_GAME2048) return fail(EPB_ERR_INVALID, "not a Game2048 pool");
+  if (p->started)
+    return fail(EPB_ERR_STATE, "Game2048 boards must be set before the pool's first reset");
+  // Sixteen tiles of 2^26 merge into 2^30 at most: every reachable tile fits the
+  // info:highest_tile bound (1 << 30) and the kernel's 5-bit cells.
+  auto check = [](const int32_t* v, int n) {
+    for (int i = 0; i < n; ++i)
+      if (v[i] < 0 || v[i] > kGame2048MaxCell) return false;
+    return true;
+  };
+  if ((initial16 && !check(initial16, 16)) || (replay512 && !check(replay512, 512)))
+    return fail(EPB_ERR_INVALID, "Game2048 board cells must be tile exponents in [0, 26]");
+  // packed as in jumanji.cu: cell c of a board at bit 5 * (c % 6) of word c / 6
+  std::vector<int32_t> cfg(kGame2048ConfigWords, 0);
+  auto pack = [&](const int32_t* b, int32_t* w) {
+    for (int c = 0; c < 16; ++c) w[c / 6] |= b[c] << (5 * (c % 6));
+  };
+  if (initial16) pack(initial16, cfg.data());
+  if (replay512)
+    for (int k = 0; k < 32; ++k) pack(replay512 + 16 * k, cfg.data() + 3 + 3 * k);
+  DeviceGuard guard(p->cfg.device);
+  EPB_CUDA(guard.status);
+  EPB_CUDA(cudaMemcpy(p->sv.rstate, cfg.data(), 4 * cfg.size(), cudaMemcpyHostToDevice));
+  p->sv.iopt = (p->sv.iopt & 1) | (initial16 ? 2 : 0) | (replay512 ? 4 : 0);
+  return EPB_OK;
 }
 int64_t epb_launch_count(const epb_pool* p) { return p ? p->launches : 0; }
 int epb_bytes_per_env_step(const epb_pool* p) { return p ? p->bytes_per_step : 0; }

@@ -343,11 +343,21 @@ struct StepOut {
 //   static constexpr bool kRngInReset, kRngInStep;  (Mt* is NULL when false)
 //   static constexpr bool kBlockObs;                (block-cooperative obs write)
 //
-// Envs with `static constexpr bool kRecReset = true` use the reset-ahead records.
+// Envs with `static constexpr bool kRecReset = true` use the reset-ahead records; envs with
+// `static constexpr bool kResetDone = true` take `int& done` as reset's last argument.
 template <class Env, class = void>
 struct UsesRec { static constexpr bool value = false; };
 template <class Env>
 struct UsesRec<Env, typename std::enable_if<Env::kRecReset>::type> {
+  static constexpr bool value = true;
+};
+// Envs with `static constexpr bool kResetDone = true` may end an episode at its reset (a
+// configured board with no legal move): their reset takes a trailing `int& done`, and the
+// reset row then reports done = 1 with step_type 0; the next step resets again.
+template <class Env, class = void>
+struct ResetDone { static constexpr bool value = false; };
+template <class Env>
+struct ResetDone<Env, typename std::enable_if<Env::kResetDone>::type> {
   static constexpr bool value = true;
 };
 
@@ -404,7 +414,11 @@ __device__ __forceinline__ void env_step(const StateView& sv, int eid, int& flag
     } else {
       cur = 0;
       done = 0;
-      Env::reset(sv, s, Env::kRngInReset ? &rng : nullptr, so);
+      if constexpr (ResetDone<Env>::value) {
+        Env::reset(sv, s, Env::kRngInReset ? &rng : nullptr, so, done);
+      } else {
+        Env::reset(sv, s, Env::kRngInReset ? &rng : nullptr, so);
+      }
     }
     if (Env::kRngInReset || Env::kRngInStep) mt_idx = rng.idx;
   }
@@ -703,11 +717,13 @@ cudaError_t launch_refill(const LaunchArgs& a) {
   return cudaGetLastError();
 }
 
-// family entry points (classic.cu / toytext.cu / mujoco.cu)
+// family entry points (classic.cu / toytext.cu / jumanji.cu / mujoco.cu)
 launch_fn classic_step_fn(int kind, int precision);
 launch_fn classic_refill_fn(int kind, int precision);
 launch_fn classic_rollout_fn(int kind, int precision);
 launch_fn toytext_step_fn(int kind, int iopt);
 launch_fn toytext_rollout_fn(int kind, int iopt);
+launch_fn jumanji_step_fn(int kind);
+launch_fn jumanji_rollout_fn(int kind);
 
 }  // namespace epb

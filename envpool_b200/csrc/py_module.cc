@@ -1,12 +1,13 @@
 // pybind11 host modules: the drop-in replacement for the class pairs the reference
 // generates with REGISTER(m, SPEC, ENVPOOL) (envpool/core/py_envpool.h:303-332) in
-// classic_control/classic_control.cc, toy_text/toy_text.cc and mujoco/gym/mujoco_envpool.cc.
+// classic_control/classic_control.cc, toy_text/toy_text.cc, jumanji/jumanji_envpool.cc and
+// mujoco/gym/mujoco_envpool.cc.
 // Same class names (_XxxEnvSpec / _XxxEnvPool), same attributes, same tuple formats, so the
 // reference's own Python layer (envpool/python/api.py:22-41 py_env()) can sit on top of it
 // unchanged.  Everything below the boundary is the C ABI of include/envpool_b200.h --
 // no env arithmetic lives in this file.
 //
-// Built three times (one module per reference family) with -DEPB_FAMILY_* selecting the
+// Built four times (one module per reference family) with -DEPB_FAMILY_* selecting the
 // env list; see envpool_b200/_build.py.
 #include <pybind11/numpy.h>
 #include <pybind11/pybind11.h>
@@ -17,6 +18,7 @@
 #include <cstdlib>
 #include <cstdint>
 #include <memory>
+#include <sstream>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -120,11 +122,36 @@ py::tuple common_defaults() {
                         INT_MAX);
 }
 
+// Game2048's board strings (jumanji/game2048_env.h ParseBoard, parse::CsvArray): comma-separated
+// integers, the first `n` of them used, missing cells 0; a token that is not a number raises
+// ValueError, as std::stoi / std::stoll do.  Empty text = not configured (an empty vector).
+std::vector<int32_t> parse_cells(const std::string& text, int n, const char* key) {
+  std::vector<int32_t> cells;
+  if (text.empty()) return cells;
+  cells.assign(n, 0);
+  std::stringstream stream(text);
+  std::string token;
+  int index = 0;
+  while (index < n && std::getline(stream, token, ',')) {
+    try {
+      cells[index++] = static_cast<int32_t>(std::stoll(token));
+    } catch (const std::exception&) {
+      throw std::invalid_argument(std::string(key) + ": '" + token + "' is not an integer");
+    }
+  }
+  for (int32_t v : cells)
+    if (v < 0 || v > 26)
+      throw std::invalid_argument(std::string(key) + ": cell " + std::to_string(v) +
+                                  " is not a tile exponent in [0, 26]");
+  return cells;
+}
+
 class SpecBase {
  public:
   const EnvDesc* desc;
   py::tuple config_values;
   std::vector<Col> state_cols, action_cols;
+  std::vector<int32_t> game2048_initial, game2048_replay;  // parsed board strings
 
   SpecBase(const EnvDesc* d, const py::tuple& conf) : desc(d) {
     const size_t want = kNumCommon + d->cfg_keys.size();
@@ -247,6 +274,16 @@ class SpecBase {
         action_cols.push_back(colb("action", 'd', {-1, 6}, -1.0, 1.0));
         break;
       }
+      case EPB_GAME2048:  // jumanji/game2048_env.h Game2048EnvFns
+        game2048_initial = parse_cells(cfg<std::string>("game2048_initial_board"), 16,
+                                       "game2048_initial_board");
+        game2048_replay = parse_cells(cfg<std::string>("game2048_replay_boards"), 32 * 16,
+                                      "game2048_replay_boards");
+        state_cols.push_back(col("obs:board", 'i', {4, 4}));
+        state_cols.push_back(colb("obs:action_mask", 'b', {4}, 0, 1));
+        state_cols.push_back(colb("info:highest_tile", 'i', {}, 1, 1 << 30));
+        action_cols.push_back(colb("action", 'i', {-1}, 0, 3));
+        break;
     }
   }
 };
@@ -319,6 +356,7 @@ class PoolBase {
       case EPB_BLACKJACK:
         c.iopt = (spec.cfg<bool>("natural") ? 1 : 0) | (spec.cfg<bool>("sab") ? 2 : 0);
         break;
+      case EPB_GAME2048: c.iopt = spec.cfg<bool>("game2048_add_random_cell") ? 1 : 0; break;
       case EPB_HALF_CHEETAH:
         c.frame_skip = spec.cfg<int>("frame_skip");
         c.ctrl_cost_weight = spec.cfg<double>("ctrl_cost_weight");
@@ -351,6 +389,10 @@ class PoolBase {
     c.env_id_offset = env_id_offset;
     h = std::make_shared<PoolHandle>();
     check(epb_create(spec.desc->kind, &c, &h->p));
+    if (!spec.game2048_initial.empty() || !spec.game2048_replay.empty())
+      check(epb_game2048_boards(
+          h->p, spec.game2048_initial.empty() ? nullptr : spec.game2048_initial.data(),
+          spec.game2048_replay.empty() ? nullptr : spec.game2048_replay.data()));
     keys.resize(epb_num_state_keys(h->p));
     for (size_t k = 0; k < keys.size(); ++k) check(epb_state_key(h->p, (int)k, &keys[k]));
     check(epb_action_key(h->p, &act));
@@ -529,6 +571,12 @@ PYBIND11_MODULE(EPB_MODULE_NAME, m) {
   register_env<EPB_NCHAIN>(m, &desc_NChain);
   register_env<EPB_CLIFF_WALKING>(m, &desc_CliffWalking);
   register_env<EPB_BLACKJACK>(m, &desc_Blackjack);
+#elif defined(EPB_FAMILY_JUMANJI)
+  // jumanji/jumanji_envpool.cc (Game2048 only)
+  DESC(Game2048, EPB_GAME2048,
+       (S{"game2048_initial_board", "game2048_replay_boards", "game2048_add_random_cell"}),
+       { return py::make_tuple(std::string(""), std::string(""), true); });
+  register_env<EPB_GAME2048>(m, &desc_Game2048);
 #elif defined(EPB_FAMILY_MUJOCO_GYM)
   // mujoco/gym/mujoco_envpool.cc (HalfCheetah only: the one MuJoCo task on the hot path)
   DESC(GymHalfCheetah, EPB_HALF_CHEETAH,

@@ -91,6 +91,39 @@ class Discrete:
         return f"Discrete({self.n})" if self.start == 0 else f"Discrete({self.n}, start={self.start})"
 
 
+class MultiBinary:
+    """gymnasium.spaces.MultiBinary stand-in: the space of a bool column."""
+
+    def __init__(self, n):
+        self.n = n
+        self.shape = tuple(int(s) for s in np.atleast_1d(n))
+        self.dtype = np.dtype(np.int8)
+
+    def contains(self, x):
+        x = np.asarray(x)
+        return bool(x.shape == self.shape and np.all((x == 0) | (x == 1)))
+
+    def __repr__(self):
+        return f"MultiBinary({self.n})"
+
+
+class DictSpace(dict):
+    """gymnasium.spaces.Dict stand-in: a dict of sub-spaces, also reachable as `.spaces`."""
+
+    @property
+    def spaces(self):
+        return self
+
+    def __repr__(self):
+        return f"Dict({dict.__repr__(self)})"
+
+
+def dict_space():
+    """An empty gymnasium.spaces.Dict (or its stand-in), the container of a multi-key
+    observation space (envpool/python/env_spec.py observation_space)."""
+    return _gymnasium.spaces.Dict() if _gymnasium is not None else DictSpace()
+
+
 class TimeStep(NamedTuple):
     """dm_env.TimeStep stand-in (same field order)."""
     step_type: Any
@@ -150,7 +183,8 @@ def to_nested_dict(flatten_dict: Dict[str, Any], generator: type = dict) -> Dict
         segments = k.split(".")
         ptr = ret
         for s in segments[:-1]:
-            if s not in ptr:
+            keys = ptr.spaces if hasattr(ptr, "spaces") else ptr
+            if s not in keys:
                 ptr[s] = generator()
             ptr = ptr[s]
         ptr[segments[-1]] = v
@@ -192,6 +226,8 @@ def gym_spec_transform(name: str, spec: ArraySpec, spec_type: str):
                                      high=spec.maximum)
     if discrete_range is not None:
         return Discrete(discrete_range[1], discrete_range[0])
+    if np.issubdtype(spec.dtype, np.bool_):
+        return MultiBinary(shape)
     return Box(spec.minimum, spec.maximum, shape, spec.dtype)
 
 

@@ -6,8 +6,8 @@ from abc import ABC, ABCMeta
 from collections import namedtuple
 from typing import Any, Dict
 
-from .data import (ArraySpec, dm_spec_transform, gym_spec_transform, to_namedtuple,
-                   to_nested_dict)
+from .data import (ArraySpec, dict_space, dm_spec_transform, gym_spec_transform,
+                   to_namedtuple, to_nested_dict)
 
 
 def check_key_duplication(cls: str, keytype: str, keys) -> None:
@@ -73,7 +73,7 @@ class EnvSpecMixin(ABC):
         }
         if len(spec) == 1:
             return list(spec.values())[0]
-        return to_nested_dict(spec)
+        return to_nested_dict(spec, dict_space)
 
     @property
     def action_space(self):
