@@ -23,7 +23,7 @@ KINDS = {
     "CartPole": 0, "Pendulum": 1, "Acrobot": 2, "MountainCar": 3,
     "MountainCarContinuous": 4, "FrozenLake": 5, "Catch": 6, "Taxi": 7,
     "NChain": 8, "CliffWalking": 9, "Blackjack": 10, "HalfCheetah": 11,
-    "Game2048": 12,
+    "Game2048": 12, "Minesweeper": 13,
 }
 DTYPES = {0: np.int32, 1: np.float32, 2: np.float64, 3: np.bool_}
 
@@ -40,6 +40,7 @@ ABI_SYMBOLS = [
     "epb_exchange_status", "epb_exchange_slice_bytes", "epb_exchange_depth",
     "epb_step_many_timed", "epb_step_exchange_many_device", "epb_fp64_peak_gflops",
     "epb_hc_model", "epb_hc_pair_rows", "epb_exchange_trace", "epb_game2048_boards",
+    "epb_minesweeper_config",
 ]
 IPC_HANDLE_BYTES = 64
 
@@ -129,6 +130,7 @@ def load_library() -> ctypes.CDLL:
     L.epb_hc_model.argtypes = [vp, ctypes.c_int64]
     L.epb_hc_pair_rows.argtypes = [vp, ci]
     L.epb_game2048_boards.argtypes = [vp, vp, vp]
+    L.epb_minesweeper_config.argtypes = [vp, vp, vp, vp, vp]
     _lib = L
     return L
 
@@ -494,6 +496,22 @@ class CPool:
             raise ValueError("Game2048 boards: 16 initial cells and 32 x 16 replay cells")
         _check(self.lib.epb_game2048_boards(self.h, None if ini is None else ini.ctypes.data,
                                             None if rep is None else rep.ctypes.data))
+
+    def minesweeper_config(self, mines=None, replay_boards=None, replay_rewards=None,
+                           replay_done=None):
+        """Minesweeper's configuration, before the first reset: `mines` 100 cells (nonzero =
+        mine), `replay_boards` 32 boards of 100 cells, `replay_rewards` / `replay_done` 32 each
+        (used only with replay boards); None = not configured.  Replay cells outside [-1, 8]
+        raise ValueError."""
+        bufs = []
+        for v, dt, n in ((mines, np.int32, 100), (replay_boards, np.int32, 3200),
+                         (replay_rewards, np.float32, 32), (replay_done, np.uint8, 32)):
+            b = None if v is None else np.ascontiguousarray(v, dtype=dt).ravel()
+            if b is not None and b.size != n:
+                raise ValueError(f"Minesweeper config: expected {n} values, got {b.size}")
+            bufs.append(b)
+        _check(self.lib.epb_minesweeper_config(
+            self.h, *[None if b is None else b.ctypes.data for b in bufs]))
 
     def state_layout(self) -> Dict[str, int]:
         out = (ctypes.c_int64 * 12)()

@@ -80,6 +80,9 @@ struct Key {
 // Game2048's configured boards (epb_game2048_boards): initial + 32 replay boards, 3 words each
 constexpr int kGame2048ConfigWords = 3 + 32 * 3;
 constexpr int kGame2048MaxCell = 26;
+// Minesweeper's configuration (epb_minesweeper_config): flags, mine mask (4 words), 32 replay
+// boards (13 words each), 32 replay rewards, the replay done flags; laid out as jumanji.cu reads it
+constexpr int kMinesweeperConfigWords = 1 + 4 + 32 * 13 + 32 + 1;
 
 static int dtype_size(int d) { return d == EPB_F64 ? 8 : d == EPB_BOOL ? 1 : 4; }
 
@@ -271,6 +274,14 @@ int build_keys(epb_pool* p) {
       add_key(p, "obs:action_mask", EPB_BOOL, {4});
       add_key(p, "info:highest_tile", EPB_I32, {});
       p->NI = 3;
+      break;
+    case EPB_MINESWEEPER:  // jumanji/minesweeper_env.h MinesweeperEnvFns
+      add_key(p, "obs:board", EPB_I32, {10, 10});
+      add_key(p, "obs:action_mask", EPB_BOOL, {10, 10});
+      add_key(p, "obs:num_mines", EPB_I32, {});
+      add_key(p, "obs:step_count", EPB_I32, {});
+      p->NI = 17;
+      a.ndim = 1; a.shape[0] = 2; a.row_bytes = 8;  // (row, column)
       break;
     case EPB_HALF_CHEETAH:
       // mujoco/gym/half_cheetah.h:44-62
@@ -714,6 +725,10 @@ int epb_create(int kind, const epb_config* cfg, epb_pool** out) {
     delete p;
     return fail(EPB_ERR_INVALID, "Game2048 iopt (add_random_cell) must be -1, 0 or 1");
   }
+  if (kind == EPB_MINESWEEPER && iopt != 0) {  // no options: epb_minesweeper_config configures
+    delete p;
+    return fail(EPB_ERR_INVALID, "Minesweeper iopt must be -1 or 0");
+  }
   if (kind == EPB_FROZEN_LAKE && iopt != 4 && iopt != 8) {
     delete p;
     return fail(EPB_ERR_INVALID, "FrozenLake size must be 4 or 8");
@@ -738,8 +753,10 @@ int epb_create(int kind, const epb_config* cfg, epb_pool** out) {
   int64_t o_idx = o_flags + al(4 * N);
   int64_t o_ist = o_idx + al(4 * N);
   int64_t o_rst = o_ist + al(4 * N * (p->NI > 0 ? p->NI : 1));
-  // Game2048 keeps its configured boards where real-valued envs keep rstate (jumanji.cu)
-  int64_t o_mt = o_rst + al(kind == EPB_GAME2048 ? 4 * kGame2048ConfigWords
+  // Game2048 and Minesweeper keep their configuration where real-valued envs keep rstate
+  // (jumanji.cu)
+  int64_t o_mt = o_rst + al(kind == EPB_GAME2048      ? 4 * kGame2048ConfigWords
+                            : kind == EPB_MINESWEEPER ? 4 * kMinesweeperConfigWords
                                                  : (int64_t)p->real_size * N * (p->NR > 0 ? p->NR : 1));
   const bool has_rec = kind <= EPB_MOUNTAIN_CAR_CONTINUOUS;  // classic_control: record resets
   int rec_q = 16;  // records per env; ENVPOOL_B200_REC_Q = 4 | 8 | 16
@@ -833,7 +850,7 @@ int epb_create(int kind, const epb_config* cfg, epb_pool** out) {
   } else if (kind <= EPB_BLACKJACK) {
     p->step_fn = toytext_step_fn(kind, iopt);
     p->rollout_fn = toytext_rollout_fn(kind, iopt);
-  } else if (kind == EPB_GAME2048) {
+  } else if (kind == EPB_GAME2048 || kind == EPB_MINESWEEPER) {
     p->step_fn = jumanji_step_fn(kind);
     p->rollout_fn = jumanji_rollout_fn(kind);
   }
@@ -871,6 +888,7 @@ int epb_create(int kind, const epb_config* cfg, epb_pool** out) {
   if (kind == EPB_FROZEN_LAKE || (kind == EPB_CLIFF_WALKING && iopt)) b += 16 + 8;
   if (kind == EPB_NCHAIN) b += 32 + 8;
   if (kind == EPB_GAME2048) b += 3 * 16 + 8;  // 3 words per moving step (bernoulli 2, Lemire 1)
+  // Minesweeper draws only at reset (50 words); like the classic envs' reset draws, not counted
   if (kind == EPB_HALF_CHEETAH) b -= 2 * (32 - 27) * 8;  // 27 of the 32-double record are live
   p->bytes_per_step = b;
   *out = p;
@@ -1737,6 +1755,37 @@ int epb_game2048_boards(epb_pool* p, const int32_t* initial16, const int32_t* re
   EPB_CUDA(guard.status);
   EPB_CUDA(cudaMemcpy(p->sv.rstate, cfg.data(), 4 * cfg.size(), cudaMemcpyHostToDevice));
   p->sv.iopt = (p->sv.iopt & 1) | (initial16 ? 2 : 0) | (replay512 ? 4 : 0);
+  return EPB_OK;
+}
+int epb_minesweeper_config(epb_pool* p, const int32_t* mines100, const int32_t* replay_boards3200,
+                           const float* replay_rewards32, const uint8_t* replay_done32) {
+  if (!p) return fail(EPB_ERR_INVALID, "null pool");
+  if (p->kind != EPB_MINESWEEPER) return fail(EPB_ERR_INVALID, "not a Minesweeper pool");
+  if (p->started)
+    return fail(EPB_ERR_STATE, "Minesweeper configuration must be set before the pool's first reset");
+  // the kernel stores value + 1 in 4 bits: -1 (unexplored) .. 8 adjacent mines
+  for (int i = 0; replay_boards3200 && i < 32 * 100; ++i)
+    if (replay_boards3200[i] < -1 || replay_boards3200[i] > 8)
+      return fail(EPB_ERR_INVALID, "Minesweeper replay board cells must lie in [-1, 8]");
+  // packed as in jumanji.cu: word 0 the flags, mine c at bit c % 32 of word 1 + c / 32, board cell
+  // c at bits 4 * (c % 8) of word c / 8 of the board's 13
+  std::vector<uint32_t> cfg(kMinesweeperConfigWords, 0u);
+  for (int c = 0; mines100 && c < 100; ++c)
+    if (mines100[c]) {
+      cfg[1 + c / 32] |= 1u << (c % 32);
+      cfg[0] |= 1u;  // at least one mine: configured placement
+    }
+  if (replay_boards3200) cfg[0] |= 2u;
+  for (int k = 0; replay_boards3200 && k < 32; ++k)
+    for (int c = 0; c < 100; ++c)
+      cfg[5 + 13 * k + c / 8] |= (uint32_t)(replay_boards3200[100 * k + c] + 1) << (4 * (c % 8));
+  for (int k = 0; replay_boards3200 && k < 32; ++k) {
+    if (replay_rewards32) std::memcpy(&cfg[5 + 13 * 32 + k], &replay_rewards32[k], 4);
+    if (replay_done32 && replay_done32[k]) cfg[5 + 13 * 32 + 32] |= 1u << k;
+  }
+  DeviceGuard guard(p->cfg.device);
+  EPB_CUDA(guard.status);
+  EPB_CUDA(cudaMemcpy(p->sv.rstate, cfg.data(), 4 * cfg.size(), cudaMemcpyHostToDevice));
   return EPB_OK;
 }
 int64_t epb_launch_count(const epb_pool* p) { return p ? p->launches : 0; }

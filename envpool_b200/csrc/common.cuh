@@ -333,7 +333,7 @@ struct StepOut {
 };
 
 // The Env concept every family member implements:
-//   using Act = <action scalar type>;  struct State {...};
+//   using Act = <action scalar type, or ActI32x2>;  struct State {...};
 //   static void load(const StateView&, int eid, State&);
 //   static void store(const StateView&, int eid, const State&);
 //   static void reset(const StateView&, State&, Mt*, StepOut&);            // XxxEnv::Reset
@@ -433,6 +433,15 @@ __device__ __forceinline__ void env_step(const StateView& sv, int eid, int& flag
 __device__ __forceinline__ void pin_value(int32_t& v) { asm volatile("" : "+r"(v)); }
 __device__ __forceinline__ void pin_value(float& v) { asm volatile("" : "+f"(v)); }
 __device__ __forceinline__ void pin_value(double& v) { asm volatile("" : "+d"(v)); }
+
+// An action row of two int32 (Minesweeper's row and column).  Only 4-byte aligned, so a row is
+// read as two adjacent 32-bit loads and caller buffers need no 8-byte alignment.
+struct alignas(4) ActI32x2 {
+  int32_t x, y;
+};
+__device__ __forceinline__ void pin_value(ActI32x2& v) {
+  asm volatile("" : "+r"(v.x), "+r"(v.y));
+}
 
 // Single sync step of a batch: thread `row` handles env env_ids[row] (identity if NULL).
 template <class Env, int kB = kBlock>

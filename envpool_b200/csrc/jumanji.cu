@@ -1,5 +1,7 @@
-// Jumanji family: Game2048-v1, bit-exact with the reference (jumanji/game2048_env.h) including
-// the libstdc++ mt19937 distribution semantics of its random cell.  One CUDA thread per env.
+// Jumanji family: Game2048-v1 and Minesweeper-v0, bit-exact with the reference
+// (jumanji/game2048_env.h, jumanji/minesweeper_env.h) including the libstdc++ mt19937
+// distribution semantics of Game2048's random cell and Minesweeper's std::shuffle.  One CUDA
+// thread per env.  Game2048 first; Minesweeper's layout is described above its struct.
 //
 // State: the 16 tile exponents (0 = empty) at 5 bits each -- cell c = row * 4 + col lives in
 // word c / 6 at bit 5 * (c % 6) -- plus the action mask of the board in bits 20..23 of word 2.
@@ -231,9 +233,317 @@ struct Game2048 {
   }
 };
 
-launch_fn jumanji_step_fn(int kind) { return kind == 12 ? launch_step<Game2048> : nullptr; }
+// ------------------------------------------------------------------------------ Minesweeper
+// Minesweeper-v0 (jumanji/minesweeper_env.h), 10 x 10 cells, cell c = row * 10 + col.
+//
+// State, 17 istate words:
+//   words 0..12  the board, cell c at bits 4 * (c % 8) of word c / 8 as value + 1 (0 = unexplored,
+//                1..9 = 0..8 adjacent mines); bits 16..31 of word 12 hold step_count
+//   words 13..16 the mine mask, cell c at bit c % 32 of word 13 + c / 32
+// The board is stored, not derived from the mines: replay boards overwrite it with any cells.
+//
+// The step works on 100-bit bitboards (Bb: cells 0..63 in lo, 64..99 in hi).  Adjacent-mine
+// counts are four bit planes summed from the eight shifted mine masks.  Reveal (a BFS in the
+// reference) is a fixed point: the clicked cell's 8-connected component inside {unexplored,
+// no mine, count 0}, grown by one dilation per round; the cells revealed are that component
+// dilated once (or the clicked cell alone), intersected with the unexplored cells.  That set
+// does not depend on the BFS order.
+//
+// The pool's configuration sits in the state blob where real-valued envs keep rstate (capi.cu
+// epb_minesweeper_config): word 0 flags (bit 0: mines are configured, bit 1: replay is on), words
+// 1..4 the configured mine mask, 5 + 13 k .. 17 + 13 k replay board k packed as the state's words
+// 0..12, 421 + k replay reward k (float bits), 453 the replay done flags (bit k).  The flags live
+// there, not in iopt, so that a state snapshot carries the whole configuration.
+struct Bb {
+  uint64_t lo, hi;
+};
+__device__ __forceinline__ Bb operator&(Bb a, Bb b) { return {a.lo & b.lo, a.hi & b.hi}; }
+__device__ __forceinline__ Bb operator|(Bb a, Bb b) { return {a.lo | b.lo, a.hi | b.hi}; }
+__device__ __forceinline__ Bb operator^(Bb a, Bb b) { return {a.lo ^ b.lo, a.hi ^ b.hi}; }
+__device__ __forceinline__ Bb operator~(Bb a) { return {~a.lo, ~a.hi}; }
+
+struct Minesweeper {
+  using Act = ActI32x2;
+  struct State {
+    uint32_t b[13];  // board nibbles (+ step_count in b[12] >> 16)
+    uint32_t m[4];   // mine mask
+  };
+  static constexpr bool kRngInReset = true, kRngInStep = false, kBlockObs = true;
+  static constexpr int kW = 10, kCells = 100, kBoardWords = 13, kMineWords = 4;
+  static constexpr int kDefaultMines = 10, kReplaySteps = 32;
+  static constexpr int kCfgMines = 1, kCfgReplay = 5, kCfgRewards = kCfgReplay + 13 * 32,
+                       kCfgDone = kCfgRewards + 32;
+
+  static __device__ __forceinline__ void load(const StateView& sv, int e, State& s) {
+    const int64_t n = sv.n_envs;
+    const uint32_t* w = reinterpret_cast<const uint32_t*>(sv.istate);
+#pragma unroll
+    for (int k = 0; k < kBoardWords; ++k) s.b[k] = w[k * n + e];
+#pragma unroll
+    for (int k = 0; k < kMineWords; ++k) s.m[k] = w[(kBoardWords + k) * n + e];
+  }
+  static __device__ __forceinline__ void store(const StateView& sv, int e, const State& s) {
+    const int64_t n = sv.n_envs;
+    uint32_t* w = reinterpret_cast<uint32_t*>(sv.istate);
+#pragma unroll
+    for (int k = 0; k < kBoardWords; ++k) w[k * n + e] = s.b[k];
+#pragma unroll
+    for (int k = 0; k < kMineWords; ++k) w[(kBoardWords + k) * n + e] = s.m[k];
+  }
+  static __device__ __forceinline__ const uint32_t* config(const StateView& sv) {
+    return static_cast<const uint32_t*>(sv.rstate);
+  }
+
+  // ---- bitboards
+  static __device__ __forceinline__ constexpr uint64_t col_bits(int c, int base) {
+    uint64_t v = 0;
+    for (int i = 0; i < 64; ++i)
+      if (base + i < kCells && (base + i) % kW == c) v |= 1ull << i;
+    return v;
+  }
+  static constexpr uint64_t kAllHi = (1ull << (kCells - 64)) - 1;
+  template <int K>
+  static __device__ __forceinline__ Bb shl(Bb x) {  // cell c -> c + K, clipped to the board
+    return {x.lo << K, ((x.hi << K) | (x.lo >> (64 - K))) & kAllHi};
+  }
+  template <int K>
+  static __device__ __forceinline__ Bb shr(Bb x) {  // cell c -> c - K
+    return {(x.lo >> K) | (x.hi << (64 - K)), x.hi >> K};
+  }
+  // cell c gets cell c + 1 / c - 1 of its own row (0 past the edge)
+  static __device__ __forceinline__ Bb from_right(Bb x) {
+    return shr<1>(x) & Bb{~col_bits(kW - 1, 0), ~col_bits(kW - 1, 64)};
+  }
+  static __device__ __forceinline__ Bb from_left(Bb x) {
+    return shl<1>(x) & Bb{~col_bits(0, 0), ~col_bits(0, 64)};
+  }
+  // x and its 8 neighbours
+  static __device__ __forceinline__ Bb dilate(Bb x) {
+    const Bb h = x | from_right(x) | from_left(x);
+    return h | shr<kW>(h) | shl<kW>(h);
+  }
+  static __device__ __forceinline__ bool same(Bb a, Bb b) { return a.lo == b.lo && a.hi == b.hi; }
+  static __device__ __forceinline__ Bb cell_bit(int c) {
+    return {c < 64 ? 1ull << c : 0ull, c >= 64 ? 1ull << (c - 64) : 0ull};
+  }
+  static __device__ __forceinline__ Bb mines_of(const State& s) {
+    return {(uint64_t)s.m[0] | ((uint64_t)s.m[1] << 32),
+            (uint64_t)s.m[2] | ((uint64_t)s.m[3] << 32)};
+  }
+  // byte k (cells 8k .. 8k + 7) of a bitboard
+  static __device__ __forceinline__ uint32_t byte_of(Bb x, int k) {
+    return (uint32_t)((k < 8 ? x.lo >> (8 * k) : x.hi >> (8 * (k - 8))) & 0xffu);
+  }
+  // 8 bits <-> one bit per nibble (bit j <-> bit 4 j)
+  static __device__ __forceinline__ uint32_t spread8(uint32_t x) {
+    x = (x | (x << 12)) & 0x000f000fu;
+    x = (x | (x << 6)) & 0x03030303u;
+    return (x | (x << 3)) & 0x11111111u;
+  }
+  static __device__ __forceinline__ uint32_t gather8(uint32_t x) {
+    x = (x | (x >> 3)) & 0x03030303u;
+    x = (x | (x >> 6)) & 0x000f000fu;
+    return (x | (x >> 12)) & 0xffu;
+  }
+  // bit 4 j set where nibble j is 0 (an unexplored cell)
+  static __device__ __forceinline__ uint32_t zero_nibbles(uint32_t w) {
+    return ~(w | (w >> 1) | (w >> 2) | (w >> 3)) & 0x11111111u;
+  }
+  static __device__ __forceinline__ Bb unexplored(const State& s) {
+    Bb u{0ull, 0ull};
+#pragma unroll
+    for (int k = 0; k < kBoardWords; ++k) {
+      const uint64_t z = gather8(zero_nibbles(k == 12 ? (s.b[k] | 0xffff0000u) : s.b[k]));
+      if (k < 8) u.lo |= z << (8 * k);
+      else u.hi |= z << (8 * (k - 8));
+    }
+    return u;
+  }
+  // c[0..3] += x, bit-sliced
+  static __device__ __forceinline__ void add1(Bb (&c)[4], Bb x) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const Bb carry = c[k] & x;
+      c[k] = c[k] ^ x;
+      x = carry;
+    }
+  }
+
+  // MinesweeperEnv::Reveal of a valid click on unexplored `cell`: writes the revealed cells'
+  // adjacent-mine counts into the board and returns the cells still unexplored.
+  static __device__ __forceinline__ Bb reveal(State& s, Bb mines, Bb unexp, int cell) {
+    Bb cnt[4] = {{0ull, 0ull}, {0ull, 0ull}, {0ull, 0ull}, {0ull, 0ull}};
+    const Bb r = from_right(mines), l = from_left(mines);
+    add1(cnt, r);
+    add1(cnt, l);
+    add1(cnt, shl<kW>(mines));  // the row above
+    add1(cnt, shl<kW>(r));
+    add1(cnt, shl<kW>(l));
+    add1(cnt, shr<kW>(mines));  // the row below
+    add1(cnt, shr<kW>(r));
+    add1(cnt, shr<kW>(l));
+    const Bb zero = unexp & ~mines & ~(cnt[0] | cnt[1] | cnt[2] | cnt[3]);
+    const Bb seed = cell_bit(cell);
+    Bb comp = seed & zero;
+#pragma unroll 1
+    while (true) {
+      const Bb next = dilate(comp) & zero;
+      if (same(next, comp)) break;
+      comp = next;
+    }
+    const Bb rev = (dilate(comp) | seed) & unexp;
+#pragma unroll
+    for (int k = 0; k < kBoardWords; ++k) {
+      const uint32_t sel = spread8(byte_of(rev, k)) * 0xfu;
+      const uint32_t val = (spread8(byte_of(cnt[0], k)) | (spread8(byte_of(cnt[1], k)) << 1) |
+                            (spread8(byte_of(cnt[2], k)) << 2) |
+                            (spread8(byte_of(cnt[3], k)) << 3)) + 0x11111111u;
+      s.b[k] = (s.b[k] & ~sel) | (val & sel);
+    }
+    return unexp & ~rev;
+  }
+  static __device__ __forceinline__ int popc(Bb x) { return __popcll(x.lo) + __popcll(x.hi); }
+  static __device__ __forceinline__ bool bit(Bb x, int c) {
+    return ((c < 64 ? x.lo >> c : x.hi >> (c - 64)) & 1ull) != 0;
+  }
+  // std::iter_swap(front + a, front + b) on the tracked front positions, a a constant
+  static __device__ __forceinline__ void swap_front(int (&f)[kDefaultMines], int a, int b) {
+    const int va = f[a];
+    int vb = f[0];
+#pragma unroll
+    for (int q = 1; q < kDefaultMines; ++q) vb = q == b ? f[q] : vb;
+    f[a] = vb;
+#pragma unroll
+    for (int q = 0; q < kDefaultMines; ++q) f[q] = q == b ? va : f[q];
+  }
+  // The first 10 cells of std::shuffle(iota(100), gen_) (libstdc++ 13 bits/stl_algo.h): one
+  // uniform_int{0, 1} for position 1, then position pairs (i, i + 1), i = 2, 4, .., 98, from
+  // one uniform_int{0, (i + 1)(i + 2) - 1} draw x each: swap i with x / (i + 2), then i + 1
+  // with x % (i + 2).  Before its own swap position i still holds i (earlier swaps touch only
+  // positions <= their step), so for i >= 10 a swap with a front position j just sets
+  // front[j] = i and the other 90 positions need no storage.
+  static __device__ __forceinline__ Bb random_mines(Mt& rng) {
+    int f[kDefaultMines];
+#pragma unroll
+    for (int q = 0; q < kDefaultMines; ++q) f[q] = q;
+    swap_front(f, 1, rng.uniform_int(0, 1));
+#pragma unroll
+    for (int i = 2; i < kDefaultMines; i += 2) {
+      const uint32_t x = (uint32_t)rng.uniform_int(0, (i + 1) * (i + 2) - 1);
+      swap_front(f, i, (int)(x / (i + 2)));
+      swap_front(f, i + 1, (int)(x % (i + 2)));
+    }
+#pragma unroll 1
+    for (int i = kDefaultMines; i < kCells; i += 2) {
+      const uint32_t x = (uint32_t)rng.uniform_int(0, (i + 1) * (i + 2) - 1);
+      const int j = (int)(x / (uint32_t)(i + 2)), k = (int)(x % (uint32_t)(i + 2));
+#pragma unroll
+      for (int q = 0; q < kDefaultMines; ++q) f[q] = q == j ? i : f[q];
+#pragma unroll
+      for (int q = 0; q < kDefaultMines; ++q) f[q] = q == k ? i + 1 : f[q];
+    }
+    Bb m{0ull, 0ull};
+#pragma unroll
+    for (int q = 0; q < kDefaultMines; ++q) m = m | cell_bit(f[q]);
+    return m;
+  }
+
+  static __device__ __forceinline__ void reset(const StateView& sv, State& s, Mt* rng,
+                                               StepOut& so) {
+#pragma unroll
+    for (int k = 0; k < kBoardWords; ++k) s.b[k] = 0u;  // all unexplored, step_count 0
+    const uint32_t* cfg = config(sv);
+    if (cfg[0] & 1u) {
+#pragma unroll
+      for (int k = 0; k < kMineWords; ++k) s.m[k] = cfg[kCfgMines + k];
+    } else {
+      const Bb m = random_mines(*rng);
+      s.m[0] = (uint32_t)m.lo;
+      s.m[1] = (uint32_t)(m.lo >> 32);
+      s.m[2] = (uint32_t)m.hi;
+      s.m[3] = (uint32_t)(m.hi >> 32);
+    }
+    so.reward = 0.0f;
+  }
+
+  static __device__ __forceinline__ void step(const StateView& sv, State& s, Act act, int cur,
+                                              int& done, Mt*, StepOut& so) {
+    float reward = 0.0f;
+    const uint32_t* cfg = config(sv);
+    if ((cfg[0] & 2u) && cur <= kReplaySteps) {  // the replay ignores the action
+      const uint32_t* board = cfg + kCfgReplay + kBoardWords * (cur - 1);
+#pragma unroll
+      for (int k = 0; k < kBoardWords; ++k) s.b[k] = board[k];
+      reward = __uint_as_float(cfg[kCfgRewards + cur - 1]);
+      done = (cfg[kCfgDone] >> (cur - 1)) & 1u;
+    } else {
+      const int row = act.x < 0 ? 0 : (act.x > kW - 1 ? kW - 1 : act.x);
+      const int col = act.y < 0 ? 0 : (act.y > kW - 1 ? kW - 1 : act.y);
+      const int cell = row * kW + col;
+      const Bb mines = mines_of(s), unexp = unexplored(s);
+      const bool valid = bit(unexp, cell), hit = bit(mines, cell);
+      bool solved = false;
+      if (valid) {
+        // explored == 100 - num_mines  <=>  unexplored == num_mines
+        solved = popc(reveal(s, mines, unexp, cell)) == popc(mines);
+        reward = hit ? 0.0f : 1.0f;
+      }
+      done = !valid || hit || solved;
+    }
+    s.b[kBoardWords - 1] = (s.b[kBoardWords - 1] & 0xffffu) | ((uint32_t)cur << 16);
+    so.reward = reward;
+  }
+
+  // obs:num_mines and obs:step_count are one coalesced 4-byte store per thread.  The 400 B
+  // obs:board and 100 B obs:action_mask rows would be 400 B / 100 B apart across a warp's
+  // lanes, so the CTA stages its envs' board words in shared memory and writes rows
+  // [row0, min(row0 + kB, row_end)) of both columns as contiguous runs: 16-byte board chunks
+  // and 4-byte mask words, four cells each (one 16-bit half of a board word).
+  template <int kB>
+  static __device__ __forceinline__ void block_write_obs(const OutView& ov, int64_t row0,
+                                                         int64_t row_end, bool active,
+                                                         const State& s, const StepOut&) {
+    // [env][word]: 13 is odd, so the staging stores of a warp hit 32 different banks
+    __shared__ uint32_t sb[kB][kBoardWords];
+    if (active) {
+      const int64_t row = row0 + threadIdx.x;
+#pragma unroll
+      for (int k = 0; k < kBoardWords; ++k) sb[threadIdx.x][k] = s.b[k];
+      if (ov.env[2])
+        static_cast<int32_t*>(ov.env[2])[row] =
+            __popc(s.m[0]) + __popc(s.m[1]) + __popc(s.m[2]) + __popc(s.m[3]);
+      if (ov.env[3]) static_cast<int32_t*>(ov.env[3])[row] = (int)(s.b[kBoardWords - 1] >> 16);
+    }
+    __syncthreads();
+    int64_t rows = row_end - row0;
+    if (rows > kB) rows = kB;
+    constexpr int kChunks = kCells / 4;  // per row
+    const int nvec = (int)rows * kChunks;
+    int4* board = ov.env[0] ? reinterpret_cast<int4*>(static_cast<int32_t*>(ov.env[0]) +
+                                                      row0 * kCells)
+                            : nullptr;
+    uint32_t* mask = ov.env[1] ? reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(ov.env[1]) +
+                                                             row0 * kCells)
+                               : nullptr;
+    for (int v = threadIdx.x; v < nvec; v += kB) {
+      const int e = v / kChunks, j = v - e * kChunks;
+      const uint32_t h = sb[e][j >> 1] >> (16 * (j & 1));
+      const uint32_t n0 = h & 15u, n1 = (h >> 4) & 15u, n2 = (h >> 8) & 15u, n3 = (h >> 12) & 15u;
+      if (board) board[v] = make_int4((int)n0 - 1, (int)n1 - 1, (int)n2 - 1, (int)n3 - 1);
+      if (mask)
+        mask[v] = (n0 == 0u ? 1u : 0u) | (n1 == 0u ? 1u << 8 : 0u) | (n2 == 0u ? 1u << 16 : 0u) |
+                  (n3 == 0u ? 1u << 24 : 0u);
+    }
+    __syncthreads();
+  }
+};
+
+launch_fn jumanji_step_fn(int kind) {
+  return kind == 12 ? launch_step<Game2048> : kind == 13 ? launch_step<Minesweeper> : nullptr;
+}
 launch_fn jumanji_rollout_fn(int kind) {
-  return kind == 12 ? launch_rollout<Game2048> : nullptr;
+  return kind == 12 ? launch_rollout<Game2048>
+                    : kind == 13 ? launch_rollout<Minesweeper> : nullptr;
 }
 
 }  // namespace epb

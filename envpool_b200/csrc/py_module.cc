@@ -146,12 +146,77 @@ std::vector<int32_t> parse_cells(const std::string& text, int n, const char* key
   return cells;
 }
 
+// Minesweeper's config strings, read with the reference's own calls and token rules
+// (jumanji/minesweeper_env.h ParseMineLocations, jumanji/parse_utils.h CsvArray), so every string
+// the reference accepts reads identically; where std::stoi / std::stoll / std::stof throw, the
+// reference throws too, and so does this (ValueError).
+struct MinesweeperConfig {
+  std::vector<int32_t> mines;    // 100 cells, 1 = mine; empty = random placement
+  std::vector<int32_t> boards;   // 32 x 100 cells, missing ones -1
+  std::vector<float> rewards;    // 32, missing ones 0.0f
+  std::vector<uint8_t> done;     // 32, missing ones false
+  bool replay = false;           // minesweeper_replay_boards is not empty
+};
+template <typename T, typename Read>
+std::vector<T> csv_array(const std::string& text, size_t n, T fill, const char* key, Read read) {
+  std::vector<T> values(n, fill);
+  if (text.empty()) return values;
+  std::stringstream stream(text);
+  std::string token;
+  size_t index = 0;
+  while (std::getline(stream, token, ',') && index < n) {
+    try {
+      values[index++] = read(token);
+    } catch (const std::exception&) {
+      throw std::invalid_argument(std::string(key) + ": cannot read '" + token + "'");
+    }
+  }
+  return values;
+}
+MinesweeperConfig parse_minesweeper(const std::string& mines, const std::string& boards,
+                                    const std::string& rewards, const std::string& done) {
+  MinesweeperConfig c;
+  if (!mines.empty()) {
+    c.mines.assign(100, 0);
+    bool any = false;
+    std::stringstream stream(mines);
+    std::string token;
+    while (std::getline(stream, token, ',')) {
+      int location;
+      try {
+        location = std::stoi(token);
+      } catch (const std::exception&) {
+        throw std::invalid_argument("minesweeper_mine_locations: cannot read '" + token + "'");
+      }
+      if (0 <= location && location < 100) {  // others are dropped, duplicates merge
+        c.mines[location] = 1;
+        any = true;
+      }
+    }
+    if (!any) c.mines.clear();  // nothing in range: random placement, as for an empty string
+  }
+  c.boards = csv_array<int32_t>(boards, 32 * 100, -1, "minesweeper_replay_boards",
+                                [](const std::string& t) { return static_cast<int32_t>(std::stoll(t)); });
+  for (int32_t v : c.boards)
+    if (v < -1 || v > 8)
+      throw std::invalid_argument("minesweeper_replay_boards: cell " + std::to_string(v) +
+                                  " is not a Minesweeper cell in [-1, 8]");
+  c.rewards = csv_array<float>(rewards, 32, 0.0f, "minesweeper_replay_rewards",
+                               [](const std::string& t) { return std::stof(t); });
+  c.done = csv_array<uint8_t>(done, 32, 0, "minesweeper_replay_done", [](const std::string& t) {
+    return static_cast<uint8_t>(t == "1" || t == "True" || t == "true");
+  });
+  c.replay = !boards.empty();
+  return c;
+}
+
 class SpecBase {
  public:
   const EnvDesc* desc;
   py::tuple config_values;
   std::vector<Col> state_cols, action_cols;
   std::vector<int32_t> game2048_initial, game2048_replay;  // parsed board strings
+  MinesweeperConfig minesweeper;
 
   SpecBase(const EnvDesc* d, const py::tuple& conf) : desc(d) {
     const size_t want = kNumCommon + d->cfg_keys.size();
@@ -284,6 +349,17 @@ class SpecBase {
         state_cols.push_back(colb("info:highest_tile", 'i', {}, 1, 1 << 30));
         action_cols.push_back(colb("action", 'i', {-1}, 0, 3));
         break;
+      case EPB_MINESWEEPER:  // jumanji/minesweeper_env.h MinesweeperEnvFns
+        minesweeper = parse_minesweeper(cfg<std::string>("minesweeper_mine_locations"),
+                                        cfg<std::string>("minesweeper_replay_boards"),
+                                        cfg<std::string>("minesweeper_replay_rewards"),
+                                        cfg<std::string>("minesweeper_replay_done"));
+        state_cols.push_back(colb("obs:board", 'i', {10, 10}, -1, 8));
+        state_cols.push_back(colb("obs:action_mask", 'b', {10, 10}, 0, 1));
+        state_cols.push_back(colb("obs:num_mines", 'i', {}, 0, 99));
+        state_cols.push_back(colb("obs:step_count", 'i', {}, 0, 90));
+        action_cols.push_back(colb("action", 'i', {-1, 2}, 0, 9));
+        break;
     }
   }
 };
@@ -393,6 +469,12 @@ class PoolBase {
       check(epb_game2048_boards(
           h->p, spec.game2048_initial.empty() ? nullptr : spec.game2048_initial.data(),
           spec.game2048_replay.empty() ? nullptr : spec.game2048_replay.data()));
+    const MinesweeperConfig& ms = spec.minesweeper;
+    if (!ms.mines.empty() || ms.replay)
+      check(epb_minesweeper_config(h->p, ms.mines.empty() ? nullptr : ms.mines.data(),
+                                   ms.replay ? ms.boards.data() : nullptr,
+                                   ms.replay ? ms.rewards.data() : nullptr,
+                                   ms.replay ? ms.done.data() : nullptr));
     keys.resize(epb_num_state_keys(h->p));
     for (size_t k = 0; k < keys.size(); ++k) check(epb_state_key(h->p, (int)k, &keys[k]));
     check(epb_action_key(h->p, &act));
@@ -572,11 +654,19 @@ PYBIND11_MODULE(EPB_MODULE_NAME, m) {
   register_env<EPB_CLIFF_WALKING>(m, &desc_CliffWalking);
   register_env<EPB_BLACKJACK>(m, &desc_Blackjack);
 #elif defined(EPB_FAMILY_JUMANJI)
-  // jumanji/jumanji_envpool.cc (Game2048 only)
+  // jumanji/jumanji_envpool.cc (Game2048 and Minesweeper)
   DESC(Game2048, EPB_GAME2048,
        (S{"game2048_initial_board", "game2048_replay_boards", "game2048_add_random_cell"}),
        { return py::make_tuple(std::string(""), std::string(""), true); });
+  DESC(Minesweeper, EPB_MINESWEEPER,
+       (S{"minesweeper_mine_locations", "minesweeper_replay_boards", "minesweeper_replay_rewards",
+          "minesweeper_replay_done"}),
+       {
+         return py::make_tuple(std::string(""), std::string(""), std::string(""),
+                               std::string(""));
+       });
   register_env<EPB_GAME2048>(m, &desc_Game2048);
+  register_env<EPB_MINESWEEPER>(m, &desc_Minesweeper);
 #elif defined(EPB_FAMILY_MUJOCO_GYM)
   // mujoco/gym/mujoco_envpool.cc (HalfCheetah only: the one MuJoCo task on the hot path)
   DESC(GymHalfCheetah, EPB_HALF_CHEETAH,
