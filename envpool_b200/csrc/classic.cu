@@ -428,44 +428,35 @@ struct MountainCar {
   }
 };
 
-launch_fn classic_step_fn(int kind, int precision) {
-  bool f32 = precision == 1;
-  switch (kind) {
-    case 0: return f32 ? launch_step<CartPole<float>> : launch_step<CartPole<double>>;
-    case 1: return f32 ? launch_step<Pendulum<float>> : launch_step<Pendulum<double>>;
-    case 2: return f32 ? launch_step<Acrobot<float>> : launch_step<Acrobot<double>>;
-    case 3: return f32 ? launch_step<MountainCar<float, false>>
-                       : launch_step<MountainCar<double, false>>;
-    case 4: return f32 ? launch_step<MountainCar<float, true>>
-                       : launch_step<MountainCar<double, true>>;
-  }
-  return nullptr;
+template <typename R>
+using MountainCarDiscrete = MountainCar<R, false>;
+template <typename R>
+using MountainCarContinuous = MountainCar<R, true>;
+
+// The kernels of Env<float> in f32 mode, of Env<double> otherwise.
+template <template <typename> class Env>
+KindLaunch classic_launch(int precision, int) {
+  return precision == EPB_PREC_F32 ? kind_launch<Env<float>>() : kind_launch<Env<double>>();
 }
-launch_fn classic_refill_fn(int kind, int precision) {
-  bool f32 = precision == 1;
-  switch (kind) {
-    case 0: return f32 ? launch_refill<CartPole<float>> : launch_refill<CartPole<double>>;
-    case 1: return f32 ? launch_refill<Pendulum<float>> : launch_refill<Pendulum<double>>;
-    case 2: return f32 ? launch_refill<Acrobot<float>> : launch_refill<Acrobot<double>>;
-    case 3: return f32 ? launch_refill<MountainCar<float, false>>
-                       : launch_refill<MountainCar<double, false>>;
-    case 4: return f32 ? launch_refill<MountainCar<float, true>>
-                       : launch_refill<MountainCar<double, true>>;
-  }
-  return nullptr;
-}
-launch_fn classic_rollout_fn(int kind, int precision) {
-  bool f32 = precision == 1;
-  switch (kind) {
-    case 0: return f32 ? launch_rollout<CartPole<float>> : launch_rollout<CartPole<double>>;
-    case 1: return f32 ? launch_rollout<Pendulum<float>> : launch_rollout<Pendulum<double>>;
-    case 2: return f32 ? launch_rollout<Acrobot<float>> : launch_rollout<Acrobot<double>>;
-    case 3: return f32 ? launch_rollout<MountainCar<float, false>>
-                       : launch_rollout<MountainCar<double, false>>;
-    case 4: return f32 ? launch_rollout<MountainCar<float, true>>
-                       : launch_rollout<MountainCar<double, true>>;
-  }
-  return nullptr;
-}
+template <template <typename> class Env>
+constexpr int kReals = kStateWords<Env<float>>;
+
+constexpr EnvKey kContinuousAction = {"action", EPB_F32, 1, {1}};
+
+// Pendulum's iopt is its version, which none of its kernels reads.
+const KindDesc kClassicKinds[] = {
+    {.kind = EPB_CARTPOLE, .keys = {{"obs", EPB_F32, 1, {4}}}, .action = kDiscreteAction,
+     .NR = kReals<CartPole>, .launch = classic_launch<CartPole>},
+    {.kind = EPB_PENDULUM, .keys = {{"obs", EPB_F32, 1, {3}}}, .action = kContinuousAction,
+     .NR = kReals<Pendulum>, .launch = classic_launch<Pendulum>},
+    {.kind = EPB_ACROBOT, .keys = {{"obs", EPB_F32, 1, {6}}, {"info:state", EPB_F32, 1, {2}}},
+     .action = kDiscreteAction, .NR = kReals<Acrobot>, .launch = classic_launch<Acrobot>},
+    {.kind = EPB_MOUNTAIN_CAR, .keys = {{"obs", EPB_F32, 1, {2}}}, .action = kDiscreteAction,
+     .NR = kReals<MountainCarDiscrete>, .launch = classic_launch<MountainCarDiscrete>},
+    {.kind = EPB_MOUNTAIN_CAR_CONTINUOUS, .keys = {{"obs", EPB_F32, 1, {2}}},
+     .action = kContinuousAction, .NR = kReals<MountainCarContinuous>,
+     .launch = classic_launch<MountainCarContinuous>},
+};
+const KindDesc* classic_kind(int kind) { return find_kind(kClassicKinds, kind); }
 
 }  // namespace epb

@@ -15,7 +15,9 @@
 #include <stdlib.h>
 
 #include <type_traits>
+#include <vector>
 
+#include "../../include/envpool_b200.h"
 #include "exchange.cuh"
 
 namespace epb {
@@ -639,6 +641,7 @@ struct LaunchArgs {
   cudaStream_t stream;
   const PeerView* peers;  // device pointer; non-NULL = fused peer exchange epilogue
   const void* next_action;  // step chains: action row of the following step (L2 prefetch)
+  const void* params;       // the pool's family parameters (KindDesc::setup; HalfCheetah only)
 };
 typedef cudaError_t (*launch_fn)(const LaunchArgs&);
 
@@ -726,13 +729,80 @@ cudaError_t launch_refill(const LaunchArgs& a) {
   return cudaGetLastError();
 }
 
-// family entry points (classic.cu / toytext.cu / jumanji.cu / mujoco.cu)
-launch_fn classic_step_fn(int kind, int precision);
-launch_fn classic_refill_fn(int kind, int precision);
-launch_fn classic_rollout_fn(int kind, int precision);
-launch_fn toytext_step_fn(int kind, int iopt);
-launch_fn toytext_rollout_fn(int kind, int iopt);
-launch_fn jumanji_step_fn(int kind);
-launch_fn jumanji_rollout_fn(int kind);
+// ---------------------------------------------------------------------------------------
+// Host description of one env kind, defined in the translation unit of its Env struct:
+// everything the engine (capi.cu) needs to lay out, validate and launch a pool of that kind.
+
+// An output or action column: enum epb_dtype, trailing dims after the batch dim.
+struct EnvKey {
+  const char* name;
+  int dtype, ndim, shape[3];
+};
+
+// The kernels of one (precision, iopt) configuration of a kind.
+struct KindLaunch {
+  launch_fn step, rollout;
+  launch_fn refill;      // non-NULL: resets come from the reset-ahead records (StateView::rec)
+  bool peer_epilogue;    // the step kernel forwards its rows to the peers (exchange.cuh)
+  // added to bytes_per_env_step's count of action, state and columns: per-step RNG traffic,
+  // less any state words a step does not touch
+  int extra_step_bytes;
+};
+
+struct KindDesc {
+  int kind;             // enum epb_kind
+  EnvKey keys[5];       // env columns after the 8 common ones (unused entries: name NULL)
+  EnvKey action;
+  int NR, NI;           // real / int32 state words per env
+  int config_words;     // int32 configuration words kept where rstate would be (0: rstate)
+  bool fp64_only;       // the precision option is ignored
+  int default_iopt;     // taken when iopt < 0
+  int iopts[2], n_iopts;  // accepted iopt values (n_iopts = 0: any value)
+  const char* iopt_error;
+  KindLaunch (*launch)(int precision, int iopt);  // precision: enum epb_precision
+  // Per-pool setup on the pool's device (NULL: none): uploads what the kernels read from
+  // device symbols and fills `params`, which LaunchArgs::params then points at.
+  cudaError_t (*setup)(const epb_config& cfg, std::vector<char>& params);
+};
+
+constexpr EnvKey kDiscreteAction = {"action", EPB_I32, 0, {}};
+
+template <class Env>
+constexpr int kStateWords = (int)(sizeof(typename Env::State) / sizeof(int32_t));
+
+template <class Env>
+KindLaunch kind_launch(int extra_step_bytes = 0) {
+  launch_fn refill = nullptr;
+  if constexpr (UsesRec<Env>::value) refill = launch_refill<Env>;
+  return {launch_step<Env>, launch_rollout<Env>, refill, true, extra_step_bytes};
+}
+// the launch of a kind whose kernels depend on neither precision nor iopt
+template <class Env, int kExtraStepBytes = 0>
+KindLaunch fixed_launch(int, int) {
+  return kind_launch<Env>(kExtraStepBytes);
+}
+
+template <size_t K>
+const KindDesc* find_kind(const KindDesc (&table)[K], int kind) {
+  for (const KindDesc& d : table)
+    if (d.kind == kind) return &d;
+  return nullptr;
+}
+
+// The kind's descriptor in the family's table, or NULL when the family does not have the kind
+// (classic.cu / toytext.cu / jumanji.cu / mujoco.cu).
+const KindDesc* classic_kind(int kind);
+const KindDesc* toytext_kind(int kind);
+const KindDesc* jumanji_kind(int kind);
+const KindDesc* mujoco_kind(int kind);
+
+// Jumanji configurations (jumanji.cu), packed into the config words its kernels read.  Either
+// argument may be NULL (not configured).  They return NULL, or the error when a cell is out of
+// range; game2048_config also sets the configured-board bits of `iopt`.
+const char* game2048_config(const int32_t* initial16, const int32_t* replay512,
+                            std::vector<uint32_t>& words, int32_t& iopt);
+const char* minesweeper_config(const int32_t* mines100, const int32_t* replay_boards3200,
+                               const float* replay_rewards32, const uint8_t* replay_done32,
+                               std::vector<uint32_t>& words);
 
 }  // namespace epb

@@ -5,8 +5,8 @@
 //
 // State: the 16 tile exponents (0 = empty) at 5 bits each -- cell c = row * 4 + col lives in
 // word c / 6 at bit 5 * (c % 6) -- plus the action mask of the board in bits 20..23 of word 2.
-// Exponents stay <= 30: configured cells are at most 26 (capi.cu), and sixteen tiles of 2^26
-// merge into one tile of 2^30 at most, so 5 bits hold every reachable tile.
+// Exponents stay <= 30: configured cells are at most 26 (game2048_config), and sixteen tiles of
+// 2^26 merge into one tile of 2^30 at most, so 5 bits hold every reachable tile.
 //
 // Each step computes the four directions once, for the board it leaves behind: that gives the
 // action mask (written out, and stored in the state) and `done` (no direction moves).  The next
@@ -14,8 +14,10 @@
 //
 // The pool's configured boards (game2048_initial_board, game2048_replay_boards) sit in the
 // state blob where real-valued envs keep rstate, packed like the state: words 0..2 the initial
-// board, words 3 + 3 k .. 5 + 3 k replay board k (capi.cu epb_game2048_boards).  iopt bit 0 is
+// board, words 3 + 3 k .. 5 + 3 k replay board k (game2048_config below).  iopt bit 0 is
 // add_random_cell, bit 1 "an initial board is configured", bit 2 "replay boards are configured".
+#include <cstring>
+
 #include "common.cuh"
 
 namespace epb {
@@ -26,6 +28,7 @@ struct Game2048 {
   static constexpr bool kRngInReset = true, kRngInStep = true, kBlockObs = false;
   static constexpr bool kResetDone = true;  // a configured board may have no legal move
   static constexpr int kReplaySteps = 32;
+  static constexpr int kConfigWords = 3 + 3 * kReplaySteps, kMaxConfigCell = 26;
 
   static __device__ __forceinline__ void load(const StateView& sv, int e, State& s) {
     const int64_t n = sv.n_envs;
@@ -249,8 +252,8 @@ struct Game2048 {
 // dilated once (or the clicked cell alone), intersected with the unexplored cells.  That set
 // does not depend on the BFS order.
 //
-// The pool's configuration sits in the state blob where real-valued envs keep rstate (capi.cu
-// epb_minesweeper_config): word 0 flags (bit 0: mines are configured, bit 1: replay is on), words
+// The pool's configuration sits in the state blob where real-valued envs keep rstate
+// (minesweeper_config below): word 0 flags (bit 0: mines are configured, bit 1: replay is on), words
 // 1..4 the configured mine mask, 5 + 13 k .. 17 + 13 k replay board k packed as the state's words
 // 0..12, 421 + k replay reward k (float bits), 453 the replay done flags (bit k).  The flags live
 // there, not in iopt, so that a state snapshot carries the whole configuration.
@@ -272,7 +275,7 @@ struct Minesweeper {
   static constexpr int kW = 10, kCells = 100, kBoardWords = 13, kMineWords = 4;
   static constexpr int kDefaultMines = 10, kReplaySteps = 32;
   static constexpr int kCfgMines = 1, kCfgReplay = 5, kCfgRewards = kCfgReplay + 13 * 32,
-                       kCfgDone = kCfgRewards + 32;
+                       kCfgDone = kCfgRewards + 32, kConfigWords = kCfgDone + 1;
 
   static __device__ __forceinline__ void load(const StateView& sv, int e, State& s) {
     const int64_t n = sv.n_envs;
@@ -538,12 +541,74 @@ struct Minesweeper {
   }
 };
 
-launch_fn jumanji_step_fn(int kind) {
-  return kind == 12 ? launch_step<Game2048> : kind == 13 ? launch_step<Minesweeper> : nullptr;
+const char* game2048_config(const int32_t* initial16, const int32_t* replay512,
+                            std::vector<uint32_t>& words, int32_t& iopt) {
+  auto check = [](const int32_t* v, int n) {
+    for (int i = 0; i < n; ++i)
+      if (v[i] < 0 || v[i] > Game2048::kMaxConfigCell) return false;
+    return true;
+  };
+  if ((initial16 && !check(initial16, 16)) || (replay512 && !check(replay512, 16 * 32)))
+    return "Game2048 board cells must be tile exponents in [0, 26]";
+  words.assign(Game2048::kConfigWords, 0u);
+  auto pack = [](const int32_t* b, uint32_t* w) {
+    for (int c = 0; c < 16; ++c) w[c / 6] |= (uint32_t)b[c] << (5 * (c % 6));
+  };
+  if (initial16) pack(initial16, words.data());
+  for (int k = 0; replay512 && k < Game2048::kReplaySteps; ++k)
+    pack(replay512 + 16 * k, words.data() + 3 + 3 * k);
+  iopt = (iopt & 1) | (initial16 ? 2 : 0) | (replay512 ? 4 : 0);
+  return nullptr;
 }
-launch_fn jumanji_rollout_fn(int kind) {
-  return kind == 12 ? launch_rollout<Game2048>
-                    : kind == 13 ? launch_rollout<Minesweeper> : nullptr;
+
+const char* minesweeper_config(const int32_t* mines100, const int32_t* replay_boards3200,
+                               const float* replay_rewards32, const uint8_t* replay_done32,
+                               std::vector<uint32_t>& words) {
+  using M = Minesweeper;
+  // the kernel stores value + 1 in 4 bits: -1 (unexplored) .. 8 adjacent mines
+  for (int i = 0; replay_boards3200 && i < M::kReplaySteps * M::kCells; ++i)
+    if (replay_boards3200[i] < -1 || replay_boards3200[i] > 8)
+      return "Minesweeper replay board cells must lie in [-1, 8]";
+  words.assign(M::kConfigWords, 0u);
+  for (int c = 0; mines100 && c < M::kCells; ++c)
+    if (mines100[c]) {
+      words[M::kCfgMines + c / 32] |= 1u << (c % 32);
+      words[0] |= 1u;  // at least one mine: configured placement
+    }
+  if (replay_boards3200) words[0] |= 2u;
+  for (int k = 0; replay_boards3200 && k < M::kReplaySteps; ++k) {
+    for (int c = 0; c < M::kCells; ++c)
+      words[M::kCfgReplay + M::kBoardWords * k + c / 8] |=
+          (uint32_t)(replay_boards3200[M::kCells * k + c] + 1) << (4 * (c % 8));
+    if (replay_rewards32) std::memcpy(&words[M::kCfgRewards + k], &replay_rewards32[k], 4);
+    if (replay_done32 && replay_done32[k]) words[M::kCfgDone] |= 1u << k;
+  }
+  return nullptr;
 }
+
+// The entries' order is the order in which the kernels are instantiated, and the code ptxas
+// makes for Minesweeper's 128-thread step kernel depends on it: reordering them changes SASS.
+const KindDesc kJumanjiKinds[] = {
+    // jumanji/minesweeper_env.h MinesweeperEnvFns.  No options: minesweeper_config configures.
+    // Draws only at reset (50 words): like the classic envs' reset draws, not counted.
+    {.kind = EPB_MINESWEEPER,
+     .keys = {{"obs:board", EPB_I32, 2, {Minesweeper::kW, Minesweeper::kW}},
+              {"obs:action_mask", EPB_BOOL, 2, {Minesweeper::kW, Minesweeper::kW}},
+              {"obs:num_mines", EPB_I32, 0, {}}, {"obs:step_count", EPB_I32, 0, {}}},
+     .action = {"action", EPB_I32, 1, {2}},  // (row, column)
+     .NI = Minesweeper::kBoardWords + Minesweeper::kMineWords,
+     .config_words = Minesweeper::kConfigWords, .iopts = {0}, .n_iopts = 1,
+     .iopt_error = "Minesweeper iopt must be -1 or 0", .launch = fixed_launch<Minesweeper>},
+    // jumanji/game2048_env.h Game2048EnvFns::StateSpec; iopt: add_random_cell
+    {.kind = EPB_GAME2048,
+     .keys = {{"obs:board", EPB_I32, 2, {4, 4}}, {"obs:action_mask", EPB_BOOL, 1, {4}},
+              {"info:highest_tile", EPB_I32, 0, {}}},
+     .action = kDiscreteAction, .NI = kStateWords<Game2048>,
+     .config_words = Game2048::kConfigWords, .default_iopt = 1, .iopts = {0, 1}, .n_iopts = 2,
+     .iopt_error = "Game2048 iopt (add_random_cell) must be -1, 0 or 1",
+     // 3 words per moving step (bernoulli 2, Lemire 1)
+     .launch = fixed_launch<Game2048, 3 * 16 + 8>},
+};
+const KindDesc* jumanji_kind(int kind) { return find_kind(kJumanjiKinds, kind); }
 
 }  // namespace epb

@@ -244,7 +244,7 @@ constexpr int kPairBlock = 64;  // threads per CTA = 32 envs
 constexpr int kPairKsMin = 9;   // fewest constraint rows per lane ever held in shared memory
 static_assert(kPairBlock == HCP_SSTRIDE, "row interleave stride = threads per CTA");
 
-// the two LegModel tables in global memory (written once per process, mjc_pool_create): every
+// the two LegModel tables in global memory (written at every pool creation, hc_setup): every
 // CTA copies them into shared memory with one coalesced read
 __device__ LegModel g_leg_model[2];
 
@@ -389,36 +389,32 @@ hc_pair_kernel(StateView sv, OutView ov, HcParams prm, const double* __restrict_
   if (side == 0) sv.flags[eid] = flags;
 }
 
-}  // namespace
-
-struct MjcPool {
-  HcParams prm;
-  int num_envs;
-};
-
-MjcPool* mjc_pool_create(int num_envs, int precision, int frame_skip, double ctrl_cost_weight,
-                         double forward_reward_weight, double reset_noise_scale) {
-  (void)precision;  // HalfCheetah always computes in fp64 (DESIGN.md)
+// On the pool's device (a second GPU needs its own copy of the symbols): the model, the leg
+// tables and the kernel's shared-memory limit; the pool's HcParams from its configuration.
+cudaError_t hc_setup(const epb_config& cfg, std::vector<char>& params) {
   static HcModel host_model;
   compile_half_cheetah(&host_model);
-  if (cudaMemcpyToSymbol(cm, &host_model, sizeof(HcModel)) != cudaSuccess) return nullptr;
+  cudaError_t e = cudaMemcpyToSymbol(cm, &host_model, sizeof(HcModel));
   LegModel legs[2];
   hcm::leg_model_of(host_model, 0, &legs[0]);
   hcm::leg_model_of(host_model, 1, &legs[1]);
   const int smem_max = hcp::MAXR * hcp::NF * kPairBlock * (int)sizeof(double);
-  if (cudaMemcpyToSymbol(g_leg_model, legs, sizeof(legs)) != cudaSuccess ||
-      cudaFuncSetAttribute(hc_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           smem_max) != cudaSuccess)
-    return nullptr;
-  MjcPool* m = new MjcPool();
-  m->num_envs = num_envs;
-  m->prm.frame_skip = frame_skip;
-  m->prm.ctrl_cost_weight = ctrl_cost_weight;
-  m->prm.forward_reward_weight = forward_reward_weight;
-  m->prm.reset_noise_scale = reset_noise_scale;
-  return m;
+  if (e == cudaSuccess) e = cudaMemcpyToSymbol(g_leg_model, legs, sizeof(legs));
+  if (e == cudaSuccess)
+    e = cudaFuncSetAttribute(hc_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             smem_max);
+  HcParams prm;
+  prm.frame_skip = cfg.frame_skip > 0 ? cfg.frame_skip : 5;
+  prm.ctrl_cost_weight = cfg.ctrl_cost_weight >= 0 ? cfg.ctrl_cost_weight : 0.1;
+  prm.forward_reward_weight = cfg.forward_reward_weight >= 0 ? cfg.forward_reward_weight : 1.0;
+  prm.reset_noise_scale = cfg.reset_noise_scale >= 0 ? cfg.reset_noise_scale : 0.1;
+  params.resize(sizeof(prm));
+  memcpy(params.data(), &prm, sizeof(prm));
+  return e;
 }
-void mjc_pool_destroy(MjcPool* m) { delete m; }
+
+}  // namespace
+
 // The compiled model as a flat blob (hcm::HcModel): host-only, for the CPU tests that run the
 // pair-lane algorithm on host threads.
 int64_t mjc_model_blob(void* dst, int64_t cap) {
@@ -429,8 +425,6 @@ int64_t mjc_model_blob(void* dst, int64_t cap) {
   }
   return (int64_t)sizeof(HcModel);
 }
-int mjc_state_reals(const MjcPool*) { return kStateReals; }
-
 // Rows per lane kept in shared memory: everything (27) while one CTA per SM covers the batch,
 // less as more CTAs share an SM (at most 4: what the kernel's registers allow).
 // ENVPOOL_B200_HC_PAIR_KS overrides (A/B switch).
@@ -450,30 +444,44 @@ static int pair_rows_in_smem(int n) {
   return ks < kPairKsMin ? kPairKsMin : ks;
 }
 
-int mjc_pair_rows(const MjcPool*, int n) { return pair_rows_in_smem(n); }
+int mjc_pair_rows(int n) { return pair_rows_in_smem(n); }
 
-static cudaError_t launch_pair(MjcPool* m, const StateView& sv, const OutView& ov,
-                               const double* d_action, const int32_t* d_env_ids, int n,
-                               int force_reset, int T, cudaStream_t stream) {
+// T sync steps of n batch rows with the pool's HcParams (LaunchArgs::params)
+static cudaError_t launch_pair(const LaunchArgs& a, const int32_t* env_ids, int n,
+                               int force_reset, int T) {
   // (Carrying fewer envs per warp -- every 2nd / 4th lane pair idle, so that a warp waits for
   // the slowest of 8 / 4 envs instead of 16 in the constraint solve -- was measured.  No gain; not
   // kept.)
   const int ks = pair_rows_in_smem(n);
   const int grid = (int)((2 * (int64_t)n + kPairBlock - 1) / kPairBlock);
   const size_t smem = (size_t)ks * hcp::NF * kPairBlock * sizeof(double);
-  hc_pair_kernel<<<grid, kPairBlock, smem, stream>>>(sv, ov, m->prm, d_action, d_env_ids, n,
-                                                     force_reset, T, ks);
+  hc_pair_kernel<<<grid, kPairBlock, smem, a.stream>>>(
+      a.sv, a.ov, *static_cast<const HcParams*>(a.params), static_cast<const double*>(a.action),
+      env_ids, n, force_reset, T, ks);
   return cudaGetLastError();
 }
+static cudaError_t hc_step(const LaunchArgs& a) {
+  return launch_pair(a, a.env_ids, a.n, a.force_reset, 1);
+}
+static cudaError_t hc_rollout(const LaunchArgs& a) {
+  return launch_pair(a, nullptr, a.sv.n_envs, 0, a.T);
+}
 
-cudaError_t mjc_launch_step(MjcPool* m, const StateView& sv, const OutView& ov,
-                            const double* d_action, const int32_t* d_env_ids, int n,
-                            int force_reset, cudaStream_t stream) {
-  return launch_pair(m, sv, ov, d_action, d_env_ids, n, force_reset, 1, stream);
-}
-cudaError_t mjc_launch_rollout(MjcPool* m, const StateView& sv, const OutView& ov,
-                               const double* d_actions, int T, cudaStream_t stream) {
-  return launch_pair(m, sv, ov, d_actions, nullptr, sv.n_envs, 0, T, stream);
-}
+// mujoco/gym/half_cheetah.h:44-62.  fp64 only (DESIGN.md); the step kernel has no peer-forwarding
+// epilogue.  27 of the 32 state reals are live, so the dead 5 are taken off bytes_per_env_step.
+const KindDesc kMujocoKinds[] = {{
+    .kind = EPB_HALF_CHEETAH,
+    .keys = {{"obs", EPB_F64, 1, {17}}, {"info:reward_run", EPB_F64, 0, {}},
+             {"info:reward_ctrl", EPB_F64, 0, {}}, {"info:x_position", EPB_F64, 0, {}},
+             {"info:x_velocity", EPB_F64, 0, {}}},
+    .action = {"action", EPB_F64, 1, {NU}},
+    .NR = kStateReals,
+    .fp64_only = true,
+    .launch = [](int, int) {
+      return KindLaunch{hc_step, hc_rollout, nullptr, false, -2 * (kStateReals - 27) * 8};
+    },
+    .setup = hc_setup,
+}};
+const KindDesc* mujoco_kind(int kind) { return find_kind(kMujocoKinds, kind); }
 
 }  // namespace epb

@@ -430,27 +430,34 @@ struct Blackjack {
   }
 };
 
-launch_fn toytext_step_fn(int kind, int iopt) {
-  switch (kind) {
-    case 5: return launch_step<FrozenLake>;
-    case 6: return launch_step<Catch>;
-    case 7: return launch_step<Taxi>;
-    case 8: return launch_step<NChain>;
-    case 9: return iopt ? launch_step<CliffWalking<true>> : launch_step<CliffWalking<false>>;
-    case 10: return launch_step<Blackjack>;
-  }
-  return nullptr;
+// Per-step RNG traffic (mt19937 table and index) of the envs that draw while stepping.
+constexpr int kSlipBytes = 16 + 8;  // FrozenLake, slippery CliffWalking: one uniform_int
+constexpr int kNChainBytes = 32 + 8;  // one uniform_real
+
+KindLaunch cliffwalking_launch(int, int iopt) {  // iopt: is_slippery
+  return iopt ? kind_launch<CliffWalking<true>>(kSlipBytes) : kind_launch<CliffWalking<false>>();
 }
-launch_fn toytext_rollout_fn(int kind, int iopt) {
-  switch (kind) {
-    case 5: return launch_rollout<FrozenLake>;
-    case 6: return launch_rollout<Catch>;
-    case 7: return launch_rollout<Taxi>;
-    case 8: return launch_rollout<NChain>;
-    case 9: return iopt ? launch_rollout<CliffWalking<true>> : launch_rollout<CliffWalking<false>>;
-    case 10: return launch_rollout<Blackjack>;
-  }
-  return nullptr;
-}
+
+// The real-state column of these pools is sized by precision although NR = 0: the state
+// snapshot format keeps it.
+const KindDesc kToyTextKinds[] = {
+    {.kind = EPB_FROZEN_LAKE, .keys = {{"obs", EPB_I32, 0, {}}}, .action = kDiscreteAction,
+     .NI = kStateWords<FrozenLake>, .default_iopt = 4, .iopts = {4, 8}, .n_iopts = 2,
+     .iopt_error = "FrozenLake size must be 4 or 8",
+     .launch = fixed_launch<FrozenLake, kSlipBytes>},
+    {.kind = EPB_CATCH, .keys = {{"obs", EPB_F32, 2, {Catch::kH, Catch::kW}}},
+     .action = kDiscreteAction, .NI = kStateWords<Catch>, .launch = fixed_launch<Catch>},
+    {.kind = EPB_TAXI, .keys = {{"obs", EPB_I32, 0, {}}}, .action = kDiscreteAction,
+     .NI = kStateWords<Taxi>, .launch = fixed_launch<Taxi>},
+    {.kind = EPB_NCHAIN, .keys = {{"obs", EPB_I32, 0, {}}}, .action = kDiscreteAction,
+     .NI = kStateWords<NChain>, .launch = fixed_launch<NChain, kNChainBytes>},
+    {.kind = EPB_CLIFF_WALKING, .keys = {{"obs", EPB_I32, 0, {}}, {"info:prob", EPB_F32, 0, {}}},
+     .action = kDiscreteAction, .NI = kStateWords<CliffWalking<false>>,
+     .launch = cliffwalking_launch},
+    // iopt: natural | sab << 1
+    {.kind = EPB_BLACKJACK, .keys = {{"obs", EPB_I32, 1, {3}}}, .action = kDiscreteAction,
+     .NI = kStateWords<Blackjack>, .default_iopt = 2, .launch = fixed_launch<Blackjack>},
+};
+const KindDesc* toytext_kind(int kind) { return find_kind(kToyTextKinds, kind); }
 
 }  // namespace epb
