@@ -11,6 +11,7 @@ loading or pool creation raises.
 from __future__ import annotations
 
 import ctypes
+import math
 import os
 from typing import Dict, List, Optional
 
@@ -182,8 +183,10 @@ class CPool:
                  max_episode_steps: int = -1, iopt: int = -1, device: int = 0,
                  precision: str = "f64", env_id_offset: int = 0,
                  env_seed=None, batch_size: int = 0, frame_skip: int = 0,
-                 ctrl_cost_weight: float = -1.0, forward_reward_weight: float = -1.0,
-                 reset_noise_scale: float = -1.0):
+                 ctrl_cost_weight: float = math.nan, forward_reward_weight: float = math.nan,
+                 reset_noise_scale: float = math.nan):
+        """HalfCheetah: frame_skip <= 0 and NaN weights / noise scale select the reference
+        defaults (5, 0.1, 1.0, 0.1); every other value is used as given, negative included."""
         L = load_library()
         self.lib = L
         cfg = EpbConfig()

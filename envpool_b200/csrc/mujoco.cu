@@ -405,9 +405,10 @@ cudaError_t hc_setup(const epb_config& cfg, std::vector<char>& params) {
                              smem_max);
   HcParams prm;
   prm.frame_skip = cfg.frame_skip > 0 ? cfg.frame_skip : 5;
-  prm.ctrl_cost_weight = cfg.ctrl_cost_weight >= 0 ? cfg.ctrl_cost_weight : 0.1;
-  prm.forward_reward_weight = cfg.forward_reward_weight >= 0 ? cfg.forward_reward_weight : 1.0;
-  prm.reset_noise_scale = cfg.reset_noise_scale >= 0 ? cfg.reset_noise_scale : 0.1;
+  // NaN = default (include/envpool_b200.h); any other value, negative included, as given
+  prm.ctrl_cost_weight = std::isnan(cfg.ctrl_cost_weight) ? 0.1 : cfg.ctrl_cost_weight;
+  prm.forward_reward_weight = std::isnan(cfg.forward_reward_weight) ? 1.0 : cfg.forward_reward_weight;
+  prm.reset_noise_scale = std::isnan(cfg.reset_noise_scale) ? 0.1 : cfg.reset_noise_scale;
   params.resize(sizeof(prm));
   memcpy(params.data(), &prm, sizeof(prm));
   return e;

@@ -15,6 +15,7 @@
 
 #include <cfloat>
 #include <climits>
+#include <cmath>
 #include <cstdlib>
 #include <cstdint>
 #include <memory>
@@ -408,6 +409,11 @@ class PoolBase {
       if (!spec.cfg<bool>("exclude_current_positions_from_observation"))
         throw std::invalid_argument(
             "HalfCheetah: exclude_current_positions_from_observation=False is not accelerated");
+      // the reference takes frame_skip substeps and divides by dt = frame_skip * timestep
+      // (half_cheetah.h:151-152): no substep and a NaN reward at 0, nonsense below
+      if (spec.cfg<int>("frame_skip") < 1)
+        throw std::invalid_argument("HalfCheetah: frame_skip must be >= 1 (the reward divides "
+                                    "by dt = frame_skip * timestep)");
     }
     epb_config c{};
     c.num_envs = spec.cfg<int>("num_envs");
@@ -424,7 +430,7 @@ class PoolBase {
     c.precision = EPB_PREC_F64;
     c.iopt = -1;
     c.frame_skip = 0;
-    c.ctrl_cost_weight = c.forward_reward_weight = c.reset_noise_scale = -1.0;
+    c.ctrl_cost_weight = c.forward_reward_weight = c.reset_noise_scale = std::nan("");
     switch (spec.desc->kind) {
       case EPB_PENDULUM: c.iopt = spec.cfg<int>("version"); break;
       case EPB_FROZEN_LAKE: c.iopt = spec.cfg<int>("size"); break;
@@ -433,7 +439,7 @@ class PoolBase {
         c.iopt = (spec.cfg<bool>("natural") ? 1 : 0) | (spec.cfg<bool>("sab") ? 2 : 0);
         break;
       case EPB_GAME2048: c.iopt = spec.cfg<bool>("game2048_add_random_cell") ? 1 : 0; break;
-      case EPB_HALF_CHEETAH:
+      case EPB_HALF_CHEETAH:  // verbatim: any sign, as the reference (half_cheetah.h:89-95)
         c.frame_skip = spec.cfg<int>("frame_skip");
         c.ctrl_cost_weight = spec.cfg<double>("ctrl_cost_weight");
         c.forward_reward_weight = spec.cfg<double>("forward_reward_weight");

@@ -21,7 +21,20 @@ columns, which reassembles the full `[num_envs, ...]` batch on every rank.  Two 
 """
 from __future__ import annotations
 
+import math
 from typing import Dict, Optional, Tuple
+
+# The task kwargs a shard hands to its pool, by engine task (the keys PoolBase::Create in
+# csrc/py_module.cc maps into epb_config), plus the ones that change no output column.  An
+# explicitly passed kwarg outside this list is refused: dropping it would run the shard with
+# the default while the caller believes otherwise.
+_COMMON_KWARGS = ("max_episode_steps", "reward_threshold", "base_path")
+_TASK_KWARGS = {
+    "FrozenLake": ("size",), "Pendulum": ("version",), "CliffWalking": ("is_slippery",),
+    "Blackjack": ("natural", "sab"),
+    "HalfCheetah": ("frame_skip", "ctrl_cost_weight", "forward_reward_weight",
+                    "reset_noise_scale", "post_constraint", "gymnasium_v5_render_camera"),
+}
 
 
 def shard_range(num_envs: int, rank: int, world: int) -> Tuple[int, int]:
@@ -102,6 +115,21 @@ class ShardedPool:
         from . import _ensure_registered
 
         _ensure_registered()
+        _, spec_cls, kwargs = registry.specs[task_id]
+        engine_task = spec_cls.replace("EnvSpec", "").replace("Gym", "")
+        dropped = sorted(set(task_kwargs) - set(_COMMON_KWARGS) -
+                         set(_TASK_KWARGS.get(engine_task, ())))
+        if dropped:
+            raise ValueError(f"ShardedPool({task_id!r}) cannot carry {dropped} to its shards")
+        kwargs = {**kwargs, **task_kwargs}
+        hc = {}
+        if engine_task == "HalfCheetah":
+            hc = dict(frame_skip=kwargs.get("frame_skip", 5),
+                      ctrl_cost_weight=kwargs.get("ctrl_cost_weight", math.nan),
+                      forward_reward_weight=kwargs.get("forward_reward_weight", math.nan),
+                      reset_noise_scale=kwargs.get("reset_noise_scale", math.nan))
+            if hc["frame_skip"] < 1:   # as make(): the reward divides by frame_skip * timestep
+                raise ValueError(f"HalfCheetah: frame_skip must be >= 1, got {hc['frame_skip']}")
         self.group = group
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1
@@ -109,9 +137,6 @@ class ShardedPool:
         self.num_envs = num_envs
         if device is None:
             device = torch.cuda.current_device()
-        _, spec_cls, kwargs = registry.specs[task_id]
-        kwargs = {**kwargs, **task_kwargs}
-        engine_task = spec_cls.replace("EnvSpec", "").replace("Gym", "")
         iopt = -1
         if engine_task == "FrozenLake":
             iopt = kwargs.get("size", 4)
@@ -124,7 +149,7 @@ class ShardedPool:
         self.pool = _capi.CPool(engine_task, self.count, seed=seed,
                                 max_episode_steps=kwargs.get("max_episode_steps", -1),
                                 iopt=iopt, device=device, precision=precision,
-                                env_id_offset=self.offset)
+                                env_id_offset=self.offset, **hc)
         self.stream = torch.cuda.ExternalStream(self.pool.stream, device=f"cuda:{device}")
         self._full = None
 

@@ -146,6 +146,9 @@ struct epo_pool {
   epo_key keys[EPO_MAX_KEYS];
   int act_elem_size, act_row_elems;
   mjc_model* mj_model;
+  /* HalfCheetah's task options (half_cheetah.h:32-42, 84-95) */
+  int hc_frame_skip;
+  double hc_ctrl_cost_weight, hc_forward_reward_weight, hc_reset_noise_scale;
 };
 
 /* per-step result scratch */
@@ -625,9 +628,14 @@ static void add_key(epo_pool* p, const char* name, int elem, int row) {
 }
 
 epo_pool* epo_create(int kind, int num_envs, int seed, const int* env_seed,
-                     int max_episode_steps, int iopt) {
+                     int max_episode_steps, int iopt, int frame_skip, double ctrl_cost_weight,
+                     double forward_reward_weight, double reset_noise_scale) {
   if (kind < 0 || kind >= EPO_NUM_KINDS || num_envs <= 0) return NULL;
   epo_pool* p = (epo_pool*)calloc(1, sizeof(epo_pool));
+  p->hc_frame_skip = frame_skip;
+  p->hc_ctrl_cost_weight = ctrl_cost_weight;
+  p->hc_forward_reward_weight = forward_reward_weight;
+  p->hc_reset_noise_scale = reset_noise_scale;
   p->kind = kind;
   p->num_envs = num_envs;
   p->max_episode_steps = max_episode_steps > 0 ? max_episode_steps : INT_MAX;
@@ -743,25 +751,27 @@ static void env_step_row(epo_pool* p, int eid, int row, const void* action,
       if (reset) bj_reset(e, &o); else bj_step(e, p->iopt & 1, (p->iopt >> 1) & 1, ai[row], &o);
       break;
     case EPO_HALF_CHEETAH: {
-      /* mujoco/gym/half_cheetah.h:127-156 */
+      /* mujoco/gym/half_cheetah.h:127-156 and WriteState, :164-185 */
+      const double fwd = p->hc_forward_reward_weight;
       if (reset) {
         e->done = 0;
         e->elapsed = 0;
-        mjc_reset(p->mj_model, e->mj, 0.1, cb_uniform, cb_normal, &e->rng);
+        mjc_reset(p->mj_model, e->mj, p->hc_reset_noise_scale, cb_uniform, cb_normal, &e->rng);
         o.reward = 0.0f;
-        o.info_d[0] = 0.0; o.info_d[1] = -0.0; o.info_d[2] = 0.0; o.info_d[3] = 0.0;
+        /* WriteState(0.0, 0.0, 0.0, 0.0, true): reward_run = 0.0 * fwd (-0.0 when fwd < 0) */
+        o.info_d[0] = 0.0 * fwd; o.info_d[1] = -0.0; o.info_d[2] = 0.0; o.info_d[3] = 0.0;
       } else {
         const double* act = (const double*)action + (size_t)row * 6;
         double x_before = mjc_qpos(e->mj)[0];
-        mjc_step(p->mj_model, e->mj, act, 5);
+        mjc_step(p->mj_model, e->mj, act, p->hc_frame_skip);
         double x_after = mjc_qpos(e->mj)[0];
         double ctrl_cost = 0.0;
-        for (int k = 0; k < 6; ++k) ctrl_cost += 0.1 * act[k] * act[k];
-        double dt = 5 * 0.01;
+        for (int k = 0; k < 6; ++k) ctrl_cost += p->hc_ctrl_cost_weight * act[k] * act[k];
+        double dt = p->hc_frame_skip * 0.01;
         double xv = (x_after - x_before) / dt;
-        o.reward = (float)(xv * 1.0 - ctrl_cost);
+        o.reward = (float)(xv * fwd - ctrl_cost);
         e->done = (++e->elapsed >= ms);
-        o.info_d[0] = xv * 1.0; o.info_d[1] = -ctrl_cost;
+        o.info_d[0] = xv * fwd; o.info_d[1] = -ctrl_cost;
         o.info_d[2] = x_after; o.info_d[3] = xv;
       }
       const double* qpos = mjc_qpos(e->mj);

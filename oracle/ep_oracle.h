@@ -39,9 +39,13 @@ typedef struct epo_pool epo_pool;
 /* iopt: FrozenLake size / Pendulum version / CliffWalking is_slippery /
  * Blackjack (natural | sab<<1); -1 = reference default.
  * env_seed: optional per-env seeds (envpool/core/env.h:101-111), else seed+env_id.
- * max_episode_steps <= 0 selects INT_MAX (envpool/core/env_spec.h:31). */
+ * max_episode_steps <= 0 selects INT_MAX (envpool/core/env_spec.h:31).
+ * frame_skip, ctrl_cost_weight, forward_reward_weight, reset_noise_scale: HalfCheetah's task
+ * options (mujoco/gym/half_cheetah.h:32-42), used as given (reference defaults 5, 0.1, 1.0,
+ * 0.1); ignored by every other kind. */
 epo_pool* epo_create(int kind, int num_envs, int seed, const int* env_seed,
-                     int max_episode_steps, int iopt);
+                     int max_episode_steps, int iopt, int frame_skip, double ctrl_cost_weight,
+                     double forward_reward_weight, double reset_noise_scale);
 void epo_destroy(epo_pool* p);
 /* Forced reset of the listed envs (AsyncEnvPool::Reset, async_envpool.h:224-237);
  * env_ids NULL = all envs in order.  Output row i <-> env_ids[i]. */

@@ -41,7 +41,8 @@ def lib():
         L = ctypes.CDLL(build())
         vp, ci = ctypes.c_void_p, ctypes.c_int
         L.epo_create.restype = vp
-        L.epo_create.argtypes = [ci, ci, ci, vp, ci, ci]
+        cd = ctypes.c_double
+        L.epo_create.argtypes = [ci, ci, ci, vp, ci, ci, ci, cd, cd, cd]
         L.epo_destroy.argtypes = [vp]
         L.epo_reset.argtypes = [vp, vp, ci]
         L.epo_step.argtypes = [vp, vp, vp, ci]
@@ -79,18 +80,21 @@ def _key_dtype(name, elem_size, kind):
 
 
 class OraclePool:
-    """CPU restatement of AsyncEnvPool<Env> in sync mode."""
+    """CPU restatement of AsyncEnvPool<Env> in sync mode.  The four HalfCheetah options are
+    used as given, with the reference's defaults (half_cheetah.h:32-42)."""
 
     def __init__(self, task, num_envs, seed=42, max_episode_steps=-1, iopt=-1,
-                 env_seed=None):
+                 env_seed=None, frame_skip=5, ctrl_cost_weight=0.1, forward_reward_weight=1.0,
+                 reset_noise_scale=0.1):
         self.kind = KINDS[task]
         self.n = num_envs
         es = None
         if env_seed is not None:
             self._env_seed = np.ascontiguousarray(env_seed, dtype=np.int32)
             es = self._env_seed.ctypes.data
-        self.h = lib().epo_create(self.kind, num_envs, seed, es,
-                                  max_episode_steps, iopt)
+        self.h = lib().epo_create(self.kind, num_envs, seed, es, max_episode_steps, iopt,
+                                  frame_skip, ctrl_cost_weight, forward_reward_weight,
+                                  reset_noise_scale)
         if not self.h:
             raise RuntimeError(f"epo_create({task}) failed")
         L = lib()

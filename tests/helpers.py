@@ -76,3 +76,58 @@ def assert_batch_equal(got, want, task, float_atol=0.0, ctx=""):
                 i = np.unravel_index(np.argmax(err - tol), err.shape)
                 raise AssertionError(f"{ctx} key {k}: |err|={err[i]:.3e} > tol at {i} "
                                      f"got {g[i]} want {w[i]}")
+
+
+# HalfCheetah's task options (half_cheetah.h:32-42).  A table rather than a product: every value
+# below appears in at least one row, and the first row is the reference default.
+#   frame_skip            1, 2, 5, 7
+#   forward_reward_weight 1.0, 0.0, -1.0, 2.5, -0.0
+#   ctrl_cost_weight      0.1, 0.0, -0.05, 1e-3
+#   reset_noise_scale     0.1, 0.0, 1.0, -0.1   (1.0 starts joints past their limits and the
+#                                                torso in the floor: constraint rows from step 1)
+HC_OPTIONS = [
+    dict(frame_skip=5, forward_reward_weight=1.0, ctrl_cost_weight=0.1, reset_noise_scale=0.1),
+    dict(frame_skip=1, forward_reward_weight=0.0, ctrl_cost_weight=0.0, reset_noise_scale=0.0),
+    dict(frame_skip=2, forward_reward_weight=-1.0, ctrl_cost_weight=-0.05, reset_noise_scale=1.0),
+    dict(frame_skip=7, forward_reward_weight=2.5, ctrl_cost_weight=1e-3, reset_noise_scale=-0.1),
+    dict(frame_skip=1, forward_reward_weight=-0.0, ctrl_cost_weight=1e-3, reset_noise_scale=1.0),
+    dict(frame_skip=2, forward_reward_weight=2.5, ctrl_cost_weight=0.0, reset_noise_scale=-0.1),
+]
+HC_DEFAULT = HC_OPTIONS[0]
+
+
+def hc_options_id(o):
+    return ("fs{frame_skip}-fwd{forward_reward_weight:g}-ctrl{ctrl_cost_weight:g}"
+            "-noise{reset_noise_scale:g}").format(**o)
+
+
+def assert_hc_env_algebra(out, x_before, action, opts, ctx=""):
+    """HalfCheetahEnv::Step's env-layer algebra (half_cheetah.h:142-160) bit for bit on every row
+    of one step's outputs `out`, from qpos[0] before the step and the raw (unclamped) actions:
+        x_velocity  = (x_position - x_before) / (frame_skip * timestep)
+        reward_run  = x_velocity * forward_reward_weight
+        reward_ctrl = -sum_k (ctrl_cost_weight * a_k) * a_k, from 0.0 in k order
+        reward      = float32(reward_run + reward_ctrl)
+    Rows that reset instead (elapsed_step 0) carry WriteState(0, 0, 0, 0): reward_run is
+    0.0 * forward_reward_weight, so -0.0 for a negative weight.  The engine and numpy do the same
+    IEEE operations in the same order, so the bytes (signs of zero included) must agree."""
+    fwd, wc = opts["forward_reward_weight"], opts["ctrl_cost_weight"]
+    stepped = out["elapsed_step"] > 0
+    a = np.asarray(action, dtype=np.float64)
+    xv = np.where(stepped, (out["info:x_position"] - x_before) / (opts["frame_skip"] * 0.01), 0.0)
+    ctrl = np.zeros(len(a))
+    for k in range(a.shape[1]):
+        ctrl = ctrl + (wc * a[:, k]) * a[:, k]
+    ctrl = np.where(stepped, ctrl, 0.0)
+    run = xv * fwd
+    want = {"info:x_velocity": xv, "info:reward_run": run, "info:reward_ctrl": -ctrl,
+            "reward": np.where(stepped, (run + -ctrl).astype(np.float32), np.float32(0.0)),
+            "info:x_position": np.where(stepped, out["info:x_position"], 0.0)}
+    for k, w in want.items():
+        g = out[k]
+        w = np.ascontiguousarray(w, dtype=g.dtype)
+        if g.tobytes() != w.tobytes():
+            bad = np.nonzero(g.view(np.uint8).reshape(len(g), -1) !=
+                             w.view(np.uint8).reshape(len(w), -1))[0][:3]
+            raise AssertionError(f"{ctx} {k} at rows {bad.tolist()}: got {g[bad].tolist()} "
+                                 f"want {w[bad].tolist()}")

@@ -9,8 +9,12 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_engine_builds_and_exports_all_declared_symbols(engine_built):
+def test_engine_exports_every_declared_symbol_at_abi_version_3(engine_built):
+    """Version 3: a NaN HalfCheetah weight or noise scale in epb_config selects the default, and
+    every other value, negative included, is used as given (up to version 2 any negative value
+    selected the default).  The header, the library and the pybind modules must agree on it."""
     from envpool_b200 import _capi
+    from envpool_b200.classic_control import classic_control_envpool
 
     hdr = open(os.path.join(ROOT, "include", "envpool_b200.h")).read()
     declared = set(re.findall(r"\b(epb_[a-z_0-9]+)\s*\(", hdr))
@@ -19,7 +23,9 @@ def test_engine_builds_and_exports_all_declared_symbols(engine_built):
     lib = ctypes.CDLL(_capi.ENGINE_SO)
     for sym in sorted(declared):
         assert hasattr(lib, sym), f"missing export {sym}"
-    assert lib.epb_abi_version() == 2
+    assert lib.epb_abi_version() == 3
+    assert re.search(r"#define EPB_ABI_VERSION (\d+)", hdr).group(1) == "3"
+    assert classic_control_envpool.__abi_version__ == 3
 
 
 def test_engine_is_sm_90a_sass():

@@ -6,6 +6,8 @@ envpool/mujoco/gym/half_cheetah.h:136-177."""
 import numpy as np
 import pytest
 
+from helpers import HC_OPTIONS, assert_hc_env_algebra, hc_options_id
+
 
 @pytest.fixture()
 def sim():
@@ -194,3 +196,63 @@ def test_newton_solver_reaches_the_minimiser_of_the_stated_problem(sim):
             trial, len(D), np.linalg.norm(a - ref.x))
         checked += 1
     assert checked >= 40, checked
+
+
+@pytest.mark.parametrize("opts", HC_OPTIONS, ids=hc_options_id)
+def test_oracle_runs_the_task_options(opts):
+    """OraclePool with HalfCheetah's task options: every step equals MjcSim stepped by hand
+    frame_skip times from the same state, bit for bit, and the env-layer algebra holds exactly
+    on the oracle's own outputs.  max_episode_steps 12 puts an auto-reset (with this reset noise
+    scale) inside the 20 steps."""
+    import ctypes
+
+    from oracle.oracle_lib import MjcSim, OraclePool, lib
+
+    n, T = 6, 20
+    p = OraclePool("HalfCheetah", n, seed=4, max_episode_steps=12, **opts)
+    scale = opts["reset_noise_scale"]
+    out = p.reset()
+    assert np.abs(out["obs"][:, :8]).max() <= abs(scale)       # qpos[1:] ~ U(-s, s)
+    if scale == 0.0:
+        assert not out["obs"].view(np.uint64).any()             # +0.0, bit for bit
+    else:
+        assert np.abs(out["obs"][:, 8:]).max() > abs(scale)     # N(0, s) has tails past |s|
+    L = lib()
+    L.mjc_warm_mut.restype = ctypes.POINTER(ctypes.c_double)
+    L.mjc_warm_mut.argtypes = [ctypes.c_void_p]
+    sim = MjcSim()
+    warm = np.ctypeslib.as_array(L.mjc_warm_mut(sim.d), shape=(9,))
+    rng = np.random.default_rng(2)
+    resets = 0
+    for t in range(T):
+        before = np.array([p.mjc_get(e) for e in range(n)])
+        a = rng.uniform(-1.5, 1.5, (n, 6))
+        out = p.step(a)
+        assert_hc_env_algebra(out, before[:, 0], a, opts, ctx=f"t={t}")
+        resets += int((out["elapsed_step"] == 0).sum())
+        for e in np.nonzero(out["elapsed_step"] > 0)[0]:
+            sim.qpos[:], sim.qvel[:], warm[:] = before[e, :9], before[e, 9:18], before[e, 18:]
+            sim.step(a[e], opts["frame_skip"])
+            np.testing.assert_array_equal(p.mjc_get(e), np.r_[sim.qpos, sim.qvel, warm])
+            np.testing.assert_array_equal(out["obs"][e], np.r_[sim.qpos[1:], sim.qvel])
+    assert resets == n
+
+
+def test_default_options_reproduce_the_recorded_outputs():
+    """A HalfCheetah OraclePool left at its default options gives, byte for byte, the outputs the
+    oracle gave when the options were still constants: sha256 over every column of two resets
+    and 25 steps (a truncation and an auto-reset among them), recorded then."""
+    import hashlib
+
+    from oracle.oracle_lib import OraclePool
+
+    p = OraclePool("HalfCheetah", 16, seed=7, max_episode_steps=20)
+    rng = np.random.default_rng(21)
+    outs = [p.reset(), p.reset()]
+    outs += [p.step(rng.uniform(-1.5, 1.5, size=(16, 6))) for _ in range(25)]
+    h = hashlib.sha256()
+    for o in outs:
+        for k in sorted(o):
+            h.update(k.encode())
+            h.update(np.ascontiguousarray(o[k]).tobytes())
+    assert h.hexdigest() == "89f0d446e730be3ba622b28a01f3a3b0cd3c4d7d76fac9799439d60cb97d2f63"

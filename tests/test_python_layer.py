@@ -97,3 +97,19 @@ def test_adapter_folds_without_a_device(engine_built):
     assert ts.last().tolist() == [False, True, True] and ts.mid().tolist() == [True, False, False]
     with pytest.raises(RuntimeError):
         CartPoleDMEnvPool.xla(None)
+
+
+def test_halfcheetah_refuses_frame_skip_below_one(engine_built):
+    """The reference takes frame_skip substeps and divides by dt = frame_skip * timestep
+    (half_cheetah.h:151-152): 0 gives a NaN reward, so the pool refuses it (and anything below)
+    before it touches a device."""
+    import warnings
+
+    import envpool_b200 as ep
+
+    for make in (ep.make_gym, ep.make_gymnasium, ep.make_dm):
+        for fs in (0, -1):
+            with warnings.catch_warnings():
+                warnings.simplefilter("ignore")
+                with pytest.raises(ValueError, match="frame_skip"):
+                    make("HalfCheetah-v4", num_envs=2, frame_skip=fs)

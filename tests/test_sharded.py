@@ -74,3 +74,20 @@ def test_two_rank_gloo_all_gather_reassembles_full_batch():
         p.join(120)
         assert p.exitcode == 0
     assert ret[0] is True and ret[1] is True
+
+
+def test_sharded_pool_refuses_kwargs_it_cannot_carry(engine_built):
+    """A task kwarg a shard's pool cannot take is refused, not dropped (the shard would run the
+    default while the caller believes otherwise); so is HalfCheetah's frame_skip < 1, as make()
+    refuses it.  All of it is decided before a device is touched."""
+    from envpool_b200.sharded import ShardedPool
+
+    for task, kw in (("Game2048-v1", dict(game2048_add_random_cell=False)),
+                     ("Minesweeper-v0", dict(minesweeper_mine_locations="0,1,2")),
+                     ("HalfCheetah-v4", dict(frame_stack=2)),
+                     ("HalfCheetah-v4", dict(exclude_current_positions_from_observation=False)),
+                     ("CartPole-v1", dict(frame_skip=2)),
+                     ("HalfCheetah-v4", dict(frame_skip=0)),
+                     ("HalfCheetah-v5", dict(frame_skip=-1))):
+        with pytest.raises(ValueError):
+            ShardedPool(task, 64, **kw)
