@@ -858,6 +858,42 @@ void epo_set_state(epo_pool* p, int eid, const double* s5, int done, int cur) {
   e->current_step = cur;
   e->elapsed = cur;
 }
+void epo_set_int_states(epo_pool* p, const int32_t* i8, const int32_t* player32,
+                        const int32_t* nplayer, const int32_t* dealer32, const int32_t* ndealer,
+                        const int32_t* done, const int32_t* cur) {
+  for (int eid = 0; eid < p->num_envs; ++eid) {
+    epo_env* e = &p->envs[eid];
+    for (int k = 0; k < 8; ++k) e->i[k] = i8[(size_t)eid * 8 + k];
+    if (player32) {
+      e->nplayer = nplayer[eid];
+      e->ndealer = ndealer[eid];
+      for (int k = 0; k < 32; ++k) {
+        e->player[k] = player32[(size_t)eid * 32 + k];
+        e->dealer[k] = dealer32[(size_t)eid * 32 + k];
+      }
+    }
+    e->done = done[eid];
+    e->current_step = cur[eid];
+    e->elapsed = cur[eid];
+  }
+}
+void epo_get_int_states(const epo_pool* p, int32_t* i8, int32_t* player32, int32_t* nplayer,
+                        int32_t* dealer32, int32_t* ndealer, int32_t* done, int32_t* cur) {
+  for (int eid = 0; eid < p->num_envs; ++eid) {
+    const epo_env* e = &p->envs[eid];
+    for (int k = 0; k < 8; ++k) i8[(size_t)eid * 8 + k] = e->i[k];
+    if (player32) {
+      nplayer[eid] = e->nplayer;
+      ndealer[eid] = e->ndealer;
+      for (int k = 0; k < 32; ++k) {
+        player32[(size_t)eid * 32 + k] = e->player[k];
+        dealer32[(size_t)eid * 32 + k] = e->dealer[k];
+      }
+    }
+    done[eid] = e->done;
+    cur[eid] = e->current_step;
+  }
+}
 void epo_mjc_set(epo_pool* p, int eid, const double* s27, int done, int cur) {
   epo_env* e = &p->envs[eid];
   memcpy(mjc_qpos_mut(e->mj), s27, sizeof(double) * 9);
@@ -883,6 +919,11 @@ void epo_debug_set_rng(epo_pool* p, int eid, const uint32_t* mt624, int idx) {
   r->idx = idx;
   r->norm_has_saved = 0;
   r->norm_saved = 0.0;
+}
+void epo_debug_get_rng(const epo_pool* p, int eid, uint32_t* mt624, int* idx) {
+  const epo_rng* r = &p->envs[eid].rng;
+  memcpy(mt624, r->mt, sizeof(r->mt));
+  *idx = r->idx;
 }
 int epo_debug_uniform_int(epo_pool* p, int eid, int a, int b) {
   return rng_uniform_int(&p->envs[eid].rng, a, b);

@@ -68,12 +68,23 @@ void epo_get_state(const epo_pool* p, int eid, double* s5, int* done, int* cur);
 void epo_set_state(epo_pool* p, int eid, const double* s5, int done, int cur);
 /* s[0..4] of every env at once: s5 is [num_envs][5] */
 void epo_get_states(const epo_pool* p, double* s5);
+/* toy_text teacher forcing of a whole pool (tests), RNG untouched: i8 is [num_envs][8]
+ * integer state i[], done / cur one per env (elapsed_step_ = current_step_ = cur).  Blackjack's
+ * hands: player32 / dealer32 [num_envs][32] cards with nplayer / ndealer counts; player32 NULL
+ * leaves the hands (and the other three hand pointers unread) alone.  The getter fills the
+ * same arrays. */
+void epo_set_int_states(epo_pool* p, const int32_t* i8, const int32_t* player32,
+                        const int32_t* nplayer, const int32_t* dealer32, const int32_t* ndealer,
+                        const int32_t* done, const int32_t* cur);
+void epo_get_int_states(const epo_pool* p, int32_t* i8, int32_t* player32, int32_t* nplayer,
+                        int32_t* dealer32, int32_t* ndealer, int32_t* done, int32_t* cur);
 /* HalfCheetah teacher forcing: s27 = qpos[9] qvel[9] qacc_warmstart[9] */
 void epo_mjc_set(epo_pool* p, int eid, const double* s27, int done, int cur);
 void epo_mjc_get(const epo_pool* p, int eid, double* s27);
 /* raw engine draw from env `eid`'s std::mt19937 (for RNG known-answer tests) */
 uint32_t epo_debug_draw(epo_pool* p, int eid);
 void epo_debug_set_rng(epo_pool* p, int eid, const uint32_t* mt624, int idx);
+void epo_debug_get_rng(const epo_pool* p, int eid, uint32_t* mt624, int* idx);
 int epo_debug_uniform_int(epo_pool* p, int eid, int a, int b);
 double epo_debug_uniform_real(epo_pool* p, int eid, double a, double b);
 double epo_debug_normal(epo_pool* p, int eid, double mean, double stddev);

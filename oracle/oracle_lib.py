@@ -62,6 +62,10 @@ def lib():
         L.epo_mjc_get.argtypes = [vp, ci, vp]
         L.epo_debug_draw.restype = ctypes.c_uint32
         L.epo_debug_draw.argtypes = [vp, ci]
+        L.epo_debug_set_rng.argtypes = [vp, ci, vp, ci]
+        L.epo_debug_get_rng.argtypes = [vp, ci, vp, vp]
+        L.epo_set_int_states.argtypes = [vp] * 8
+        L.epo_get_int_states.argtypes = [vp] * 8
         _lib = L
     return _lib
 
@@ -162,6 +166,45 @@ class OraclePool:
         out = np.zeros((self.n, 5))
         lib().epo_get_states(self.h, out.ctypes.data)
         return out
+
+    def set_int_states(self, st):
+        """toy_text: overwrite every env's integer state at once, RNG untouched.  `st` is a
+        dict of int32 arrays as int_states() returns: i [N, 8], done [N], cur [N] and, for
+        Blackjack, player / dealer [N, 32] with nplayer / ndealer [N]."""
+        a = {k: np.ascontiguousarray(v, dtype=np.int32) for k, v in st.items()}
+        assert a["i"].shape == (self.n, 8) and a["done"].shape == a["cur"].shape == (self.n,)
+        hands = "player" in a
+        if hands:
+            assert a["player"].shape == a["dealer"].shape == (self.n, 32)
+        ptr = lambda k: a[k].ctypes.data if k in a else None  # noqa: E731
+        lib().epo_set_int_states(self.h, ptr("i"), ptr("player"), ptr("nplayer"),
+                                 ptr("dealer"), ptr("ndealer"), ptr("done"), ptr("cur"))
+
+    def int_states(self):
+        """Every env's integer state, done flag and step counter (the layout set_int_states
+        takes); Blackjack's hands too."""
+        n = self.n
+        st = {"i": np.zeros((n, 8), np.int32), "done": np.zeros(n, np.int32),
+              "cur": np.zeros(n, np.int32)}
+        if self.kind == KINDS["Blackjack"]:
+            st.update(player=np.zeros((n, 32), np.int32), dealer=np.zeros((n, 32), np.int32),
+                      nplayer=np.zeros(n, np.int32), ndealer=np.zeros(n, np.int32))
+        ptr = lambda k: st[k].ctypes.data if k in st else None  # noqa: E731
+        lib().epo_get_int_states(self.h, ptr("i"), ptr("player"), ptr("nplayer"),
+                                 ptr("dealer"), ptr("ndealer"), ptr("done"), ptr("cur"))
+        return st
+
+    def set_rng(self, eid, mt624, idx):
+        """Load env `eid`'s std::mt19937: 624 table words and the read position (624 = the
+        next draw regenerates the table)."""
+        row = np.ascontiguousarray(mt624, dtype=np.uint32)
+        assert row.shape == (624,)
+        lib().epo_debug_set_rng(self.h, eid, row.ctypes.data, int(idx))
+
+    def rng(self, eid):
+        mt, idx = np.zeros(624, np.uint32), ctypes.c_int()
+        lib().epo_debug_get_rng(self.h, eid, mt.ctypes.data, ctypes.byref(idx))
+        return mt, idx.value
 
     def mjc_set(self, eid, s27, done, cur):
         buf = np.ascontiguousarray(s27, dtype=np.float64)

@@ -131,11 +131,14 @@ def test_f32_mode_free_running_short_horizon(capi, task):
     assert in_sync.mean() >= 0.98, in_sync.mean()
 
 
-@pytest.mark.parametrize("task", ["CartPole", "FrozenLake", "Catch", "Blackjack", "Acrobot"])
+@pytest.mark.parametrize("task", ["CartPole", "FrozenLake", "Catch", "Blackjack", "Acrobot",
+                                  "Taxi", "NChain", "CliffWalking", "CliffWalking-slippery"])
 def test_device_path_and_rollout_match_host_path(capi, task):
     import torch
 
+    task, _, slippery = task.partition("-")
     ms, iopt = REGISTERED[task]
+    iopt = 1 if slippery else iopt
     N, T = 3000, 40   # not a multiple of the CTA size: exercises the tail CTA
     rng = np.random.default_rng(2)
     acts = random_actions(task, rng, (T, N))
@@ -205,7 +208,8 @@ def test_env_seed_list_and_errors(capi):
         pool.recv()                                       # nothing outstanding
 
 
-@pytest.mark.parametrize("task", ["FrozenLake", "CartPole", "Pendulum"])
+@pytest.mark.parametrize("task", ["FrozenLake", "CartPole", "Pendulum", "Catch", "Taxi", "NChain",
+                                  "CliffWalking", "Blackjack"])
 def test_snapshot_roundtrip(capi, task):
     """The state blob is the whole env state (classic_control: the reset-ahead records
     travel with it)."""

@@ -7,54 +7,17 @@ tests/test_oracle_rng_vs_libstdcxx.py pins those branches of the ORACLE against 
 itself on the CPU; here the same crafted states are loaded into the engine
 (epb_state_import) and into the oracle (epo_debug_set_rng) and both must keep agreeing.
 
-Crafting: a table whose words 0..8 are zero and whose words 397..404 are the untempered
-wanted outputs makes the next regeneration of chunk 0 (device: mt_idx = 0; std::mt19937:
-position 624) emit exactly those outputs; every later chunk regenerates identically on both
-sides because the whole 624-word table is the same."""
-import ctypes
-
+Crafting (toy_text_cases.crafted_table): a table whose words 0..8 are zero and whose words
+397..404 are the untempered wanted outputs makes the next regeneration of chunk 0 (device:
+mt_idx = 0; std::mt19937: position 624) emit exactly those outputs; every later chunk
+regenerates identically on both sides because the whole 624-word table is the same."""
 import numpy as np
 import pytest
 
 from helpers import assert_batch_equal
-from test_oracle_rng_vs_libstdcxx import untemper
+from toy_text_cases import crafted_table, load_both
 
 pytestmark = pytest.mark.gpu
-
-
-def crafted_table(rng, outputs):
-    mt = rng.integers(0, 2**32, size=624, dtype=np.uint32)
-    mt[0:9] = 0
-    for k, v in enumerate(outputs):
-        mt[397 + k] = untemper(v)
-    return mt
-
-
-def load_both(pool, orc, tables, force_done):
-    """tables: [N, 624] uint32.  Engine: chunked [78][N][8], mt_idx = 0; oracle: position 624."""
-    from oracle import oracle_lib
-
-    L = oracle_lib.lib()
-    L.epo_debug_set_rng.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int]
-    blob = pool.state_export()
-    st = pool.state_arrays(blob)
-    n = tables.shape[0]
-    st["mt"][:] = tables.reshape(n, 78, 8).transpose(1, 0, 2)
-    st["mt_idx"][:] = 0
-    if "rprod" in st:
-        # classic_control keeps each env's NEXT initial states in a ring of records drawn from
-        # the table before the crafting; emptying the ring makes epb_state_import redraw all
-        # of them from the crafted table (the refill path), as the oracle's next Resets will
-        st["rprod"][:] = st["rcons"]
-    if force_done:
-        st["flags"][:] = st["flags"] | 1
-    pool.state_import(blob)
-    for e in range(n):
-        row = np.ascontiguousarray(tables[e])
-        L.epo_debug_set_rng(orc.h, e, row.ctypes.data, 624)
-        if force_done:
-            s5, _, cur = orc.get_state(e)
-            orc.set_state(e, s5, 1, cur)
 
 
 def patterns(rng, n, rejected):

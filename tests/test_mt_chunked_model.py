@@ -156,7 +156,7 @@ def test_crafted_table_emits_wanted_words_in_both_representations():
     import ctypes
 
     from oracle import oracle_lib
-    from test_gpu_rng_corner_cases import crafted_table
+    from toy_text_cases import crafted_table
 
     L = oracle_lib.lib()
     L.epo_debug_set_rng.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int]
