@@ -934,3 +934,22 @@ double epo_debug_uniform_real(epo_pool* p, int eid, double a, double b) {
 double epo_debug_normal(epo_pool* p, int eid, double mean, double stddev) {
   return rng_normal(&p->envs[eid].rng, mean, stddev);
 }
+int epo_trig(int kind, const void* x, int n, void* s, void* c) {
+  if (kind == 0) {
+    const double* xd = (const double*)x;
+    for (int i = 0; i < n; ++i) {
+      if (s) ((double*)s)[i] = sin(xd[i]);
+      if (c) ((double*)c)[i] = cos(xd[i]);
+    }
+    return 0;
+  }
+  if (kind == 1) {
+    const float* xf = (const float*)x;
+    for (int i = 0; i < n; ++i) {
+      if (s) ((float*)s)[i] = sinf(xf[i]);
+      if (c) ((float*)c)[i] = cosf(xf[i]);
+    }
+    return 0;
+  }
+  return -1;
+}

@@ -89,6 +89,11 @@ int epo_debug_uniform_int(epo_pool* p, int eid, int a, int b);
 double epo_debug_uniform_real(epo_pool* p, int eid, double a, double b);
 double epo_debug_normal(epo_pool* p, int eid, double mean, double stddev);
 
+/* libm's sin and cos of n arguments, as the classic_control steps above take them: kind 0 =
+ * double sin / cos, kind 1 = float sinf / cosf (x, s, c then point to floats).  s or c may be
+ * NULL.  Returns 0, or -1 for an unknown kind. */
+int epo_trig(int kind, const void* x, int n, void* s, void* c);
+
 #ifdef __cplusplus
 }
 #endif

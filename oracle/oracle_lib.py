@@ -66,8 +66,23 @@ def lib():
         L.epo_debug_get_rng.argtypes = [vp, ci, vp, vp]
         L.epo_set_int_states.argtypes = [vp] * 8
         L.epo_get_int_states.argtypes = [vp] * 8
+        L.epo_trig.argtypes = [ci, vp, ci, vp, vp]
         _lib = L
     return _lib
+
+
+def libm_trig(x, want_sin=True, want_cos=True):
+    """libm's sin and cos of every element of `x` (float64: sin / cos, float32: sinf / cosf),
+    the functions the oracle's classic_control steps call; (sin, cos), None where not wanted.
+    numpy's own sin is not libm's, so the oracle's values come from here."""
+    x = np.ascontiguousarray(x)
+    kind = {np.dtype(np.float64): 0, np.dtype(np.float32): 1}[x.dtype]
+    s = np.empty_like(x) if want_sin else None
+    c = np.empty_like(x) if want_cos else None
+    rc = lib().epo_trig(kind, x.ctypes.data, x.size, None if s is None else s.ctypes.data,
+                        None if c is None else c.ctypes.data)
+    assert rc == 0, rc
+    return s, c
 
 
 def _key_dtype(name, elem_size, kind):

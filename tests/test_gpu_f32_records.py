@@ -21,6 +21,7 @@ entry point must give the same bits."""
 import numpy as np
 import pytest
 
+from classic_cases import Draws
 from helpers import EXACT_KEYS, REGISTERED, assert_batch_equal, random_actions
 
 pytestmark = pytest.mark.gpu
@@ -43,29 +44,6 @@ def _float_err(got, want):
             w64 = w.astype(np.float64)
             err = max(err, float((np.abs(got[k] - w64) / (1 + np.abs(w64))).max()))
     return err
-
-
-class Draws:
-    """Each env's i-th initial state, from an oracle pool stepped only by forced resets: after
-    its (i+1)-th reset it holds the state the engine's ring keeps as record i (record 0 is what
-    the engine's first forced reset consumes)."""
-
-    def __init__(self, task, n, seed, iopt, env_seed=None):
-        from oracle.oracle_lib import OraclePool
-
-        self.orc = OraclePool(task, n, seed=seed, iopt=iopt, env_seed=env_seed)
-        self.nr = NR[task]
-        self.table = np.empty((0, n, self.nr))
-
-    def upto(self, m):
-        """[>= m, n, NR] float64: records 0 .. m-1 of every env."""
-        grow = []
-        for _ in range(m - self.table.shape[0]):
-            self.orc.reset()
-            grow.append(self.orc.states()[:, :self.nr])
-        if grow:
-            self.table = np.concatenate([self.table, np.stack(grow)])
-        return self.table
 
 
 def check_rings(st, draws, count, precision, ctx, rows=slice(None), full=False):
