@@ -6,7 +6,7 @@ Produces (all git-ignored):
   envpool_b200/lib/libenvpool_b200.so      C-ABI engine (include/envpool_b200.h), sm_90a
   envpool_b200/<family>_envpool*.so        pybind11 host modules (classic_control_envpool,
                                            toy_text_envpool, jumanji_envpool,
-                                           mujoco_gym_envpool)
+                                           mujoco_gym_envpool, pgx_envpool)
 nvcc cross-compiles for sm_90a without a GPU, so this runs on a machine without one.
 """
 from __future__ import annotations
@@ -35,17 +35,20 @@ CUDA_UNITS = {
     "toytext.cu": [],
     "jumanji.cu": [],
     "mujoco.cu": [],
+    "pgx.cu": [],
     "capi.cu": [],
 }
 PY_MODULES = {
     # module name and location as in the reference (envpool/classic_control/
     # classic_control_envpool, envpool/toy_text/toy_text_envpool,
-    # envpool/jumanji/jumanji_envpool, envpool/mujoco/mujoco_gym_envpool) ->
+    # envpool/jumanji/jumanji_envpool, envpool/mujoco/mujoco_gym_envpool,
+    # envpool/pgx/pgx_envpool) ->
     # (sub-directory, family macro)
     "classic_control_envpool": ("classic_control", "EPB_FAMILY_CLASSIC_CONTROL"),
     "toy_text_envpool": ("toy_text", "EPB_FAMILY_TOY_TEXT"),
     "jumanji_envpool": ("jumanji", "EPB_FAMILY_JUMANJI"),
     "mujoco_gym_envpool": ("mujoco", "EPB_FAMILY_MUJOCO_GYM"),
+    "pgx_envpool": ("pgx", "EPB_FAMILY_PGX"),
 }
 
 

@@ -20,12 +20,16 @@ import numpy as np
 _PKG = os.path.dirname(os.path.abspath(__file__))
 ENGINE_SO = os.path.join(_PKG, "lib", "libenvpool_b200.so")
 
+# enum epb_kind of the single-player kinds
 KINDS = {
     "CartPole": 0, "Pendulum": 1, "Acrobot": 2, "MountainCar": 3,
     "MountainCarContinuous": 4, "FrozenLake": 5, "Catch": 6, "Taxi": 7,
     "NChain": 8, "CliffWalking": 9, "Blackjack": 10, "HalfCheetah": 11,
     "Game2048": 12, "Minesweeper": 13,
 }
+# ... and of the kinds with two players per env, whose per-player columns hold two rows per env
+# row (epb_state_key_players).  Kept apart: code that walks KINDS sees one-player pools only.
+TWO_PLAYER_KINDS = {"TicTacToe": 14, "ConnectFour": 15}
 DTYPES = {0: np.int32, 1: np.float32, 2: np.float64, 3: np.bool_}
 
 # every symbol include/envpool_b200.h declares (checked by tests/test_abi.py)
@@ -41,7 +45,7 @@ ABI_SYMBOLS = [
     "epb_exchange_status", "epb_exchange_slice_bytes", "epb_exchange_depth",
     "epb_step_many_timed", "epb_step_exchange_many_device", "epb_fp64_peak_gflops",
     "epb_hc_model", "epb_hc_pair_rows", "epb_exchange_trace", "epb_game2048_boards",
-    "epb_minesweeper_config",
+    "epb_minesweeper_config", "epb_state_key_players",
 ]
 IPC_HANDLE_BYTES = 64
 
@@ -86,6 +90,7 @@ def load_library() -> ctypes.CDLL:
     L.epb_destroy.argtypes = [vp]
     L.epb_num_state_keys.argtypes = [vp]
     L.epb_state_key.argtypes = [vp, ci, ctypes.POINTER(EpbKeyInfo)]
+    L.epb_state_key_players.argtypes = [vp, ci]
     L.epb_action_key.argtypes = [vp, ctypes.POINTER(EpbKeyInfo)]
     L.epb_slab_bytes.restype = ctypes.c_int64
     L.epb_slab_bytes.argtypes = [vp]
@@ -165,10 +170,16 @@ def _check(rc: int):
 
 
 class Key:
-    def __init__(self, info: EpbKeyInfo):
+    """One state or action column.  `shape` is the shape of an env row: a per-player column of a
+    multi-player pool (`players` > 1) leads with the player dimension."""
+
+    def __init__(self, info: EpbKeyInfo, players: int = 1):
         self.name = info.name.decode()
         self.dtype = np.dtype(DTYPES[info.dtype])
+        self.players = players
         self.shape = tuple(info.shape[i] for i in range(info.ndim))
+        if players > 1:
+            self.shape = (players,) + self.shape
         self.row_bytes = info.row_bytes
         self.offset = info.slab_offset
 
@@ -209,7 +220,8 @@ class CPool:
         cfg.forward_reward_weight = forward_reward_weight
         cfg.reset_noise_scale = reset_noise_scale
         h = ctypes.c_void_p()
-        _check(L.epb_create(KINDS[task], ctypes.byref(cfg), ctypes.byref(h)))
+        kind = KINDS[task] if task in KINDS else TWO_PLAYER_KINDS[task]
+        _check(L.epb_create(kind, ctypes.byref(cfg), ctypes.byref(h)))
         self.h = h
         self.task = task
         self.n = num_envs
@@ -236,7 +248,7 @@ class CPool:
         for k in range(L.epb_num_state_keys(h)):
             info = EpbKeyInfo()
             _check(L.epb_state_key(h, k, ctypes.byref(info)))
-            self.keys.append(Key(info))
+            self.keys.append(Key(info, L.epb_state_key_players(h, k)))
         info = EpbKeyInfo()
         _check(L.epb_action_key(h, ctypes.byref(info)))
         self.action_key = Key(info)

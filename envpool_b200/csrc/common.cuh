@@ -331,8 +331,50 @@ __device__ __forceinline__ void write_common(const OutView& ov, int64_t row, int
 // Per-env result of one EnvStep, kept in registers until the output write.
 struct StepOut {
   float reward;
-  float extra;  // env-specific scalar (CliffWalking info:prob)
+  float extra;  // env-specific scalar (CliffWalking info:prob; player 1's reward when P = 2)
 };
+
+// Common output columns of a kind with P = 2 players per env (Env::Allocate(2), env.h:224-256).
+// The per-player columns hold rows 2 row and 2 row + 1 for env row `row`: info:players.env_id
+// (the env's id twice), reward (players 0 and 1: so.reward, so.extra) and discount.  The
+// reference writes discount through a one-element assignment to a 2-row slice of a zero-filled
+// buffer, so player 1's discount is always 0.
+__device__ __forceinline__ void write_common_pair(const OutView& ov, int64_t row, int global_eid,
+                                                  int cur, int done, const StepOut& so,
+                                                  int max_steps) {
+  const int step_type = (cur == 0) ? 0 : (done ? 2 : 1);
+  if (ov.env_id) ov.env_id[row] = global_eid;
+  if (ov.players_id) reinterpret_cast<int2*>(ov.players_id)[row] = make_int2(global_eid, global_eid);
+  if (ov.elapsed) ov.elapsed[row] = cur;
+  if (ov.done) ov.done[row] = (uint8_t)done;
+  if (ov.reward) reinterpret_cast<float2*>(ov.reward)[row] = make_float2(so.reward, so.extra);
+  if (ov.discount)
+    reinterpret_cast<float2*>(ov.discount)[row] = make_float2(done ? 0.0f : 1.0f, 0.0f);
+  if (ov.step_type) ov.step_type[row] = step_type;
+  const int trunc = done && (cur >= max_steps);
+  if (ov.trunc) ov.trunc[row] = (uint8_t)trunc;
+  if (ov.wire) ov.wire[row] = pack_wire(cur, done, trunc);
+}
+
+// Players per env (P): 1 unless the Env declares `static constexpr int kPlayers`.  Per-player
+// output columns keep the P rows of an env row next to each other, so every row count, row
+// range and stride of the engine keeps counting env rows.
+template <class Env, class = void>
+struct Players { static constexpr int value = 1; };
+template <class Env>
+struct Players<Env, typename std::enable_if<(Env::kPlayers > 1)>::type> {
+  static constexpr int value = Env::kPlayers;
+};
+template <class Env>
+__device__ __forceinline__ void write_common_env(const OutView& ov, int64_t row, int global_eid,
+                                                 int flags, const StepOut& so, int max_steps) {
+  if constexpr (Players<Env>::value == 1) {
+    write_common(ov, row, global_eid, flags >> 1, flags & 1, so.reward, max_steps);
+  } else {
+    static_assert(Players<Env>::value == 2, "per-player columns: P = 1 or 2");
+    write_common_pair(ov, row, global_eid, flags >> 1, flags & 1, so, max_steps);
+  }
+}
 
 // The Env concept every family member implements:
 //   using Act = <action scalar type, or ActI32x2>;  struct State {...};
@@ -492,8 +534,7 @@ step_kernel(StateView sv, OutView ov, const typename Env::Act* __restrict__ acti
     Env::store(sv, eid, s);
     sv.flags[eid] = flags;
     if (!kRec && kRng && mt_idx != mt_idx0) sv.mt_idx[eid] = mt_idx;
-    write_common(ov, row, eid + sv.env_id_offset, flags >> 1, flags & 1, so.reward,
-                 sv.max_steps);
+    write_common_env<Env>(ov, row, eid + sv.env_id_offset, flags, so, sv.max_steps);
   }
   if constexpr (Env::kBlockObs) {
     Env::template block_write_obs<kB>(ov, (int64_t)blockIdx.x * kB, n, active, s, so);
@@ -593,8 +634,7 @@ rollout_kernel(StateView sv, OutView ov, const typename Env::Act* __restrict__ a
       } else {
         env_step<Env>(sv, eid, flags, s, a, false, so, mt_idx, 0);
       }
-      write_common(ov, row, eid + sv.env_id_offset, flags >> 1, flags & 1, so.reward,
-                   sv.max_steps);
+      write_common_env<Env>(ov, row, eid + sv.env_id_offset, flags, so, sv.max_steps);
     }
     if constexpr (Env::kBlockObs) {
       Env::template block_write_obs<kBlock>(
@@ -737,6 +777,7 @@ cudaError_t launch_refill(const LaunchArgs& a) {
 struct EnvKey {
   const char* name;
   int dtype, ndim, shape[3];
+  bool per_player = false;  // one row per player (KindDesc::players rows per env row)
 };
 
 // The kernels of one (precision, iopt) configuration of a kind.
@@ -763,6 +804,10 @@ struct KindDesc {
   // Per-pool setup on the pool's device (NULL: none): uploads what the kernels read from
   // device symbols and fills `params`, which LaunchArgs::params then points at.
   cudaError_t (*setup)(const epb_config& cfg, std::vector<char>& params);
+  // Players per env (the Env's Players<Env>::value).  For players > 1 the per-player columns
+  // (info:players.env_id, reward, discount and the keys marked per_player) hold that many
+  // adjacent rows per env row.
+  int players = 1;
 };
 
 constexpr EnvKey kDiscreteAction = {"action", EPB_I32, 0, {}};
@@ -790,11 +835,12 @@ const KindDesc* find_kind(const KindDesc (&table)[K], int kind) {
 }
 
 // The kind's descriptor in the family's table, or NULL when the family does not have the kind
-// (classic.cu / toytext.cu / jumanji.cu / mujoco.cu).
+// (classic.cu / toytext.cu / jumanji.cu / mujoco.cu / pgx.cu).
 const KindDesc* classic_kind(int kind);
 const KindDesc* toytext_kind(int kind);
 const KindDesc* jumanji_kind(int kind);
 const KindDesc* mujoco_kind(int kind);
+const KindDesc* pgx_kind(int kind);
 
 // Jumanji configurations (jumanji.cu), packed into the config words its kernels read.  Either
 // argument may be NULL (not configured).  They return NULL, or the error when a cell is out of

@@ -1,13 +1,13 @@
 // pybind11 host modules: the drop-in replacement for the class pairs the reference
 // generates with REGISTER(m, SPEC, ENVPOOL) (envpool/core/py_envpool.h:303-332) in
-// classic_control/classic_control.cc, toy_text/toy_text.cc, jumanji/jumanji_envpool.cc and
-// mujoco/gym/mujoco_envpool.cc.
+// classic_control/classic_control.cc, toy_text/toy_text.cc, jumanji/jumanji_envpool.cc,
+// mujoco/gym/mujoco_envpool.cc and pgx/pgx.cc.
 // Same class names (_XxxEnvSpec / _XxxEnvPool), same attributes, same tuple formats, so the
 // reference's own Python layer (envpool/python/api.py:22-41 py_env()) can sit on top of it
 // unchanged.  Everything below the boundary is the C ABI of include/envpool_b200.h --
 // no env arithmetic lives in this file.
 //
-// Built four times (one module per reference family) with -DEPB_FAMILY_* selecting the
+// Built five times (one module per reference family) with -DEPB_FAMILY_* selecting the
 // env list; see envpool_b200/_build.py.
 #include <pybind11/numpy.h>
 #include <pybind11/pybind11.h>
@@ -361,6 +361,18 @@ class SpecBase {
         state_cols.push_back(colb("obs:step_count", 'i', {}, 0, 90));
         action_cols.push_back(colb("action", 'i', {-1, 2}, 0, 9));
         break;
+      case EPB_TIC_TAC_TOE:  // pgx/board_games.h TicTacToeEnvFns
+      case EPB_CONNECT_FOUR: {  // pgx/board_games.h ConnectFourEnvFns
+        const bool ttt = desc->kind == EPB_TIC_TAC_TOE;
+        const int rows = ttt ? 3 : 6, cols = ttt ? 3 : 7, actions = ttt ? 9 : 7;
+        state_cols.push_back(col("obs", 'b', {-1, rows, cols, 2}));
+        state_cols.push_back(col("info:board", 'i', {rows, cols}));
+        state_cols.push_back(col("info:current_player", 'i', {}));
+        state_cols.push_back(col("info:legal_action_mask", 'b', {actions}));
+        state_cols.push_back(colb("info:players.id", 'i', {-1}, 0, 1));
+        action_cols.push_back(colb("action", 'i', {-1}, 0, actions - 1));
+        break;
+      }
     }
   }
 };
@@ -393,14 +405,24 @@ class PoolBase {
  public:
   std::shared_ptr<PoolHandle> h;
   std::vector<epb_key_info> keys;
+  std::vector<int> key_players;  // epb_state_key_players of each state key
+  int players = 1;               // players per env (max_num_players)
   epb_key_info act{};
   std::vector<int32_t> env_seed;
   int device_ordinal = 0;  // resolved CUDA device of the pool
 
   void Create(const SpecBase& spec, int device, const std::string& precision,
               int env_id_offset) {
-    if (spec.cfg<int>("max_num_players") != 1)
+    const bool two_players =
+        spec.desc->kind == EPB_TIC_TAC_TOE || spec.desc->kind == EPB_CONNECT_FOUR;
+    if (two_players) {
+      if (spec.cfg<int>("max_num_players") != 2)
+        throw std::invalid_argument(std::string(spec.desc->name) +
+                                    " is a two-player game: max_num_players must be 2");
+    } else if (spec.cfg<int>("max_num_players") != 1) {
       throw std::invalid_argument("max_num_players != 1 is outside the accelerated path");
+    }
+    players = two_players ? 2 : 1;
     if (spec.desc->kind == EPB_HALF_CHEETAH) {
       // post_constraint (v5) only adds mj_rnePostConstraint (mujoco_env.h:145-147), whose
       // outputs (cacc/cfrc_*) HalfCheetah never reads: accepted, no effect on any column.
@@ -482,8 +504,46 @@ class PoolBase {
                                    ms.replay ? ms.rewards.data() : nullptr,
                                    ms.replay ? ms.done.data() : nullptr));
     keys.resize(epb_num_state_keys(h->p));
-    for (size_t k = 0; k < keys.size(); ++k) check(epb_state_key(h->p, (int)k, &keys[k]));
+    key_players.resize(keys.size());
+    for (size_t k = 0; k < keys.size(); ++k) {
+      check(epb_state_key(h->p, (int)k, &keys[k]));
+      key_players[k] = epb_state_key_players(h->p, (int)k);
+      if (key_players[k] < 1) check(key_players[k]);
+    }
     check(epb_action_key(h->p, &act));
+  }
+
+  // Multi-player pools: the action row of each env row is the one of its first player row, the
+  // first i with players.env_id[i] == env_id (Env::ParseAction, core/env.h:146-176, and the
+  // `action["action"_][0]` each game's Step reads).  An env without a player row raises.
+  py::array_t<int, py::array::c_style> FirstPlayerActions(
+      const py::array_t<int, py::array::c_style | py::array::forcecast>& ids,
+      const py::array& player_env_id, const py::array& action) const {
+    py::array_t<int, py::array::c_style | py::array::forcecast> pids(player_env_id);
+    py::array_t<int, py::array::c_style | py::array::forcecast> pa(action);
+    const int m = static_cast<int>(pids.size());
+    if (static_cast<int64_t>(pa.nbytes()) != static_cast<int64_t>(m) * act.row_bytes)
+      throw std::invalid_argument("action batch does not match players.env_id batch");
+    const int num_envs = epb_num_envs(h->p);
+    std::vector<int> first(num_envs, -1);
+    const int* pid = pids.data();
+    for (int i = m - 1; i >= 0; --i)
+      if (pid[i] >= 0 && pid[i] < num_envs) first[pid[i]] = i;
+    const int n = static_cast<int>(ids.size());
+    py::array_t<int, py::array::c_style> out(n);
+    int* o = out.mutable_data();
+    const int* id = ids.data();
+    const int* av = pa.data();
+    for (int i = 0; i < n; ++i) {
+      const int e = id[i];
+      if (e < 0 || e >= num_envs)
+        throw std::invalid_argument("env_id " + std::to_string(e) + " out of range");
+      if (first[e] < 0)
+        throw std::invalid_argument("env_id " + std::to_string(e) +
+                                    " has no row in players.env_id: no action for that env");
+      o[i] = av[first[e]];
+    }
+    return out;
   }
 
   // PyEnvPool::PySend, py_envpool.h:244-250
@@ -491,7 +551,8 @@ class PoolBase {
     if (action.size() != 3) throw std::invalid_argument("expected [env_id, players.env_id, action]");
     py::array_t<int, py::array::c_style | py::array::forcecast> ids(action[0]);
     py::array a;
-    if (act.dtype == EPB_I32) a = py::array_t<int, py::array::c_style | py::array::forcecast>(action[2]);
+    if (players > 1) a = FirstPlayerActions(ids, action[1], action[2]);
+    else if (act.dtype == EPB_I32) a = py::array_t<int, py::array::c_style | py::array::forcecast>(action[2]);
     else if (act.dtype == EPB_F32) a = py::array_t<float, py::array::c_style | py::array::forcecast>(action[2]);
     else a = py::array_t<double, py::array::c_style | py::array::forcecast>(action[2]);
     int n = static_cast<int>(ids.size());
@@ -509,6 +570,8 @@ class PoolBase {
 
   // PyEnvPool::PyRecv, py_envpool.h:255-266: zero-copy numpy views over one pinned slab;
   // a capsule keeps the slab (and the pool) alive until every returned array is dropped.
+  // A per-player column comes back as [n * P, ...], the reference's player rows: the engine
+  // keeps the P rows of an env row next to each other.
   std::vector<py::array> Recv() {
     void* slab = nullptr;
     int n = 0, row0 = 0, rc;
@@ -520,10 +583,12 @@ class PoolBase {
     auto lease = std::make_shared<SlabLease>(h, slab);
     std::vector<py::array> ret;
     ret.reserve(keys.size());
-    for (const epb_key_info& k : keys) {
+    for (size_t kk = 0; kk < keys.size(); ++kk) {
+      const epb_key_info& k = keys[kk];
+      const int P = key_players[kk];
       auto* holder = new std::shared_ptr<SlabLease>(lease);
       py::capsule cap(holder, [](void* p) { delete static_cast<std::shared_ptr<SlabLease>*>(p); });
-      std::vector<py::ssize_t> shape = {n};
+      std::vector<py::ssize_t> shape = {static_cast<py::ssize_t>(n) * P};
       for (int i = 0; i < k.ndim; ++i) shape.push_back(k.shape[i]);
       char* base = static_cast<char*>(slab) + k.slab_offset +
                    static_cast<size_t>(row0) * k.row_bytes;
@@ -685,6 +750,13 @@ PYBIND11_MODULE(EPB_MODULE_NAME, m) {
                                false, 0.1, 1.0, 0.1);
        });
   register_env<EPB_HALF_CHEETAH>(m, &desc_GymHalfCheetah);
+#elif defined(EPB_FAMILY_PGX)
+  // pgx/pgx.cc (TicTacToe and ConnectFour: the two-player board games on the hot path)
+  DESC(TicTacToe, EPB_TIC_TAC_TOE, S{"task"}, { return py::make_tuple(std::string("tic_tac_toe")); });
+  DESC(ConnectFour, EPB_CONNECT_FOUR, S{"task"},
+       { return py::make_tuple(std::string("connect_four")); });
+  register_env<EPB_TIC_TAC_TOE>(m, &desc_TicTacToe);
+  register_env<EPB_CONNECT_FOUR>(m, &desc_ConnectFour);
 #else
 #error "define one EPB_FAMILY_* macro"
 #endif

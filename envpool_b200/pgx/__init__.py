@@ -1,0 +1,15 @@
+"""PGX family: binds the engine's pybind11 classes (`_TicTacToeEnvSpec` / `_TicTacToeEnvPool`,
+`_ConnectFourEnvSpec` / `_ConnectFourEnvPool`, csrc/py_module.cc) to the Python adapters and
+exports `XxxEnvSpec`, `XxxDMEnvPool` and `XxxGymnasiumEnvPool` for both -- the names
+envpool/pgx/__init__.py exports for those games.  Both are two-player pools: per-player columns
+(obs, reward, discount, info:players.env_id, info:players.id) hold two rows per env."""
+from ..python.api import py_env
+from . import pgx_envpool as _ext
+
+TicTacToeEnvSpec, TicTacToeDMEnvPool, TicTacToeGymnasiumEnvPool = py_env(
+    _ext._TicTacToeEnvSpec, _ext._TicTacToeEnvPool)
+ConnectFourEnvSpec, ConnectFourDMEnvPool, ConnectFourGymnasiumEnvPool = py_env(
+    _ext._ConnectFourEnvSpec, _ext._ConnectFourEnvPool)
+
+__all__ = ["TicTacToeEnvSpec", "TicTacToeDMEnvPool", "TicTacToeGymnasiumEnvPool",
+           "ConnectFourEnvSpec", "ConnectFourDMEnvPool", "ConnectFourGymnasiumEnvPool"]

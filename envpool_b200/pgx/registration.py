@@ -1,0 +1,10 @@
+"""PGX env registration (task ids, `task` and max_num_players as in envpool/pgx/registration.py;
+TicTacToe and ConnectFour are the accelerated PGX games)."""
+from ..registration import register
+
+register(task_id="TicTacToe-v1", import_path="envpool_b200.pgx", spec_cls="TicTacToeEnvSpec",
+         dm_cls="TicTacToeDMEnvPool", gymnasium_cls="TicTacToeGymnasiumEnvPool",
+         task="tic_tac_toe", max_num_players=2)
+register(task_id="ConnectFour-v1", import_path="envpool_b200.pgx",
+         spec_cls="ConnectFourEnvSpec", dm_cls="ConnectFourDMEnvPool",
+         gymnasium_cls="ConnectFourGymnasiumEnvPool", task="connect_four", max_num_players=2)

@@ -38,6 +38,66 @@ class EnvPoolMixin(ABC):
 
     _spec: Any
 
+    def _player_action_count(self, adict: Dict[str, Any]) -> Optional[int]:
+        """Rows of the player actions present in `adict` (envpool.py:82-101)."""
+        count = None
+        for key, spec in self.spec.action_array_spec.items():
+            if key in ("env_id", "players.env_id") or key not in adict:
+                continue
+            shape = tuple(spec.shape)
+            if len(shape) == 0 or shape[0] != -1:
+                continue
+            value_shape = np.shape(adict[key])
+            rows = 1 if len(value_shape) == 0 else int(value_shape[0])
+            if count is None:
+                count = rows
+            elif count != rows:
+                raise RuntimeError("Inconsistent leading dimensions across player actions.")
+        return count
+
+    def _cached_players_env_id(self, env_id: np.ndarray,
+                               player_count: int) -> Optional[np.ndarray]:
+        """The player rows of `env_id` in the last recv, when they number `player_count`
+        (envpool.py:103-121)."""
+        if not hasattr(self, "_last_players_env_id"):
+            return None
+        cached = self._last_players_env_id
+        segments = []
+        for eid in env_id.tolist():
+            matches = cached[cached == eid]
+            if matches.size == 0:
+                return None
+            segments.append(matches)
+        if not segments:
+            return np.empty(0, dtype=np.int32)
+        players_env_id = np.concatenate(segments)
+        if players_env_id.shape[0] != player_count:
+            return None
+        return players_env_id
+
+    def _infer_players_env_id(self, adict: Dict[str, Any]) -> np.ndarray:
+        """players.env_id when the caller gives none (envpool.py:123-149): env_id itself for
+        one action per env, else the last recv's player rows of those envs, else each env id
+        repeated once per player."""
+        env_id = _normalize_env_id(adict["env_id"])
+        max_num_players = self.config.get("max_num_players", 1)
+        if max_num_players == 1:
+            return env_id
+        player_count = self._player_action_count(adict)
+        if player_count is None or player_count == env_id.shape[0]:
+            return env_id
+        cached = self._cached_players_env_id(env_id, player_count)
+        if cached is not None:
+            return cached
+        if env_id.shape[0] == 0 or player_count % env_id.shape[0] != 0:
+            raise RuntimeError("Cannot infer players.env_id for multiplayer action; "
+                               "pass a dict action with explicit players.env_id.")
+        players_per_env = player_count // env_id.shape[0]
+        if players_per_env > max_num_players:
+            raise RuntimeError("Cannot infer players.env_id for multiplayer action; "
+                               "per-env player count exceeds max_num_players.")
+        return np.repeat(env_id, players_per_env).astype(np.int32, copy=False)
+
     def _check_action(self, actions: List[np.ndarray]) -> None:
         if hasattr(self, "_check_action_finished"):  # only check once
             return
@@ -74,7 +134,9 @@ class EnvPoolMixin(ABC):
         else:
             adict["env_id"] = _normalize_env_id(env_id)
         if "players.env_id" not in adict:
-            adict["players.env_id"] = _normalize_env_id(adict["env_id"])
+            adict["players.env_id"] = self._infer_players_env_id(adict)
+        else:
+            adict["players.env_id"] = _normalize_env_id(adict["players.env_id"])
         if not hasattr(self, "_action_names"):
             self._action_names = self._spec._action_keys
         return [adict[k] for k in self._action_names]
@@ -108,6 +170,10 @@ class EnvPoolMixin(ABC):
 
     def recv(self, reset: bool = False, return_info: bool = True):
         state_list = self._recv()
+        if self.config.get("max_num_players", 1) > 1:
+            # the player rows of this batch, for _infer_players_env_id (envpool.py:317-320)
+            k = self._spec._state_keys.index("info:players.env_id")
+            self._last_players_env_id = np.array(state_list[k], dtype=np.int32, copy=True)
         return self._to(state_list, reset, return_info)
 
     def async_reset(self) -> None:
@@ -152,7 +218,11 @@ class EnvPoolMixin(ABC):
     def step_device(self, action, env_id=None, stream=None):
         """One sync step with `action` (and optional `env_id`) already in HBM (torch CUDA
         tensors).  Returns {state_key: torch view} into the device output slab; the views
-        are valid until the next step.  No host copy happens."""
+        are valid until the next step.  No host copy happens.
+
+        `action` holds one row per env row, also in multi-player pools: there it is the action
+        of the env's player to move (the first player row, as `send` resolves it).  A
+        per-player column comes back as [n, players, ...]."""
         dp = self.device_pool
         dp.step_device(action, env_id, stream=stream)
         n = env_id.shape[0] if env_id is not None else None

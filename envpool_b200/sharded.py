@@ -34,6 +34,7 @@ _TASK_KWARGS = {
     "Blackjack": ("natural", "sab"),
     "HalfCheetah": ("frame_skip", "ctrl_cost_weight", "forward_reward_weight",
                     "reset_noise_scale", "post_constraint", "gymnasium_v5_render_camera"),
+    "TicTacToe": ("task", "max_num_players"), "ConnectFour": ("task", "max_num_players"),
 }
 
 
@@ -122,6 +123,9 @@ class ShardedPool:
         if dropped:
             raise ValueError(f"ShardedPool({task_id!r}) cannot carry {dropped} to its shards")
         kwargs = {**kwargs, **task_kwargs}
+        players = 2 if engine_task in ("TicTacToe", "ConnectFour") else 1
+        if kwargs.get("max_num_players", 1) != players:
+            raise ValueError(f"ShardedPool({task_id!r}): max_num_players must be {players}")
         hc = {}
         if engine_task == "HalfCheetah":
             hc = dict(frame_skip=kwargs.get("frame_skip", 5),
