@@ -170,14 +170,12 @@ struct epb_pool {
   bool x_ipc[kMaxPeers] = {};
   bool x_attached = false;
   long long x_timeout_ns = 10000000000LL;
-  bool x_fused = false;  // peer stores issued by the step kernel's epilogue (else push_kernel)
-  bool x_side_push = true;  // captured chains: push_kernel on the side branch, not in the chain
   long long* x_trace = nullptr;  // ENVPOOL_B200_EXCHANGE_TRACE: device timeline, 8 stamps / step
   int64_t x_trace_steps = 0;
   uint64_t x_steps = 0;   // host count of exchanged steps; step t uses slot t % D
   uint64_t x_waited = 0;  // host count of enqueued waits
   cudaStream_t x_side = nullptr;            // wait branch of the engine-captured chains
-  cudaStream_t x_push[3] = {};              // push branches (x_side_push): push(k) on k % 3
+  cudaStream_t x_push[3] = {};              // push branches of captured chains: push(k) on k % 3
   cudaEvent_t x_ev_step[kMaxDepth] = {}, x_ev_wait[kMaxDepth] = {}, x_ev_push[kMaxDepth] = {};
 
   int64_t x_mine(int slot) const { return ((int64_t)slot * x_world + x_rank) * x_slice; }
@@ -303,9 +301,10 @@ int get_event(epb_pool* p, cudaEvent_t* ev) {
   return EPB_OK;
 }
 
-// Copy the wire columns of the local slice to every peer, then publish (families without the
-// forwarding epilogue: HalfCheetah; or ENVPOOL_B200_EXCHANGE=push).  Column k is
-// ceil(n * row_bytes / 16) 16-byte units (the 256-byte column padding absorbs the tail).
+// Copy the wire columns of the local slice to every peer, then publish: behind the step for
+// kinds without the forwarding epilogue (HalfCheetah), and on the push branches of captured
+// chains for every kind.  Column k is ceil(n * row_bytes / 16) 16-byte units (the 256-byte
+// column padding absorbs the tail).
 __global__ void __launch_bounds__(256)
 push_kernel(const PeerView* __restrict__ pv, int n) {
   const int world = pv->world, rank = pv->rank;
@@ -1140,7 +1139,7 @@ int run_chain(epb_pool* p, cudaStream_t st, const ChainKey& c, bool fork, cudaEv
     if (c.exchange) {
       if (xfork && k >= D - 1)
         EPB_CUDA(cudaStreamWaitEvent(st, p->x_ev_wait[(k - (D - 1)) % D], 0));
-      if (xfork && p->x_side_push) {
+      if (xfork) {
         // The peer stores leave the step chain: step k only computes (into its local slot
         // k % D); push(k), a copy kernel on a branch of its own, sends the wire columns, and
         // wait_derive(k) follows on the wait branch.  Pipelines beside each other:
@@ -1159,14 +1158,6 @@ int run_chain(epb_pool* p, cudaStream_t st, const ChainKey& c, bool fork, cudaEv
         if (rc != EPB_OK) return rc;
         EPB_CUDA(cudaEventRecord(p->x_ev_push[k % D], ps));
         EPB_CUDA(cudaStreamWaitEvent(p->x_side, p->x_ev_push[k % D], 0));
-        rc = exchange_wait_launch(p, p->x_side);
-        if (rc != EPB_OK) return rc;
-        EPB_CUDA(cudaEventRecord(p->x_ev_wait[k % D], p->x_side));
-      } else if (xfork) {
-        rc = exchange_step(p, a, st, rec ? -2 : -1, nx);
-        if (rc != EPB_OK) return rc;
-        EPB_CUDA(cudaEventRecord(p->x_ev_step[k % D], st));
-        EPB_CUDA(cudaStreamWaitEvent(p->x_side, p->x_ev_step[k % D], 0));
         rc = exchange_wait_launch(p, p->x_side);
         if (rc != EPB_OK) return rc;
         EPB_CUDA(cudaEventRecord(p->x_ev_wait[k % D], p->x_side));
@@ -1227,7 +1218,7 @@ int chain_entry(epb_pool* p, const void* d_actions, int T_stream, int t0, int K,
   DeviceGuard guard(p->cfg.device);
   EPB_CUDA(guard.status);
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : p->stream;
-  if (exchange && use_graph && p->x_side_push && !p->x_push[0]) {
+  if (exchange && use_graph && !p->x_push[0]) {
     // push branches of the captured exchange chains: created on first use (a pool that never
     // captures one never holds them -- streams map onto a bounded set of hardware queues)
     for (cudaStream_t& ps : p->x_push) EPB_CUDA(cudaStreamCreateWithFlags(&ps, cudaStreamNonBlocking));
@@ -1255,11 +1246,7 @@ int chain_entry(epb_pool* p, const void* d_actions, int T_stream, int t0, int K,
       EPB_CUDA(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
       const int64_t before = p->launches;
       const uint64_t xs = p->x_steps, xw = p->x_waited;
-      static const bool no_fork = [] {
-        const char* e = getenv("ENVPOOL_B200_REFILL_FORK");
-        return e && e[0] == '0';
-      }();
-      int rc = run_chain(p, s, key, !no_fork, ev0, ev1);
+      int rc = run_chain(p, s, key, true, ev0, ev1);
       const int64_t launches = p->launches - before;
       p->launches = before;  // capture records, it does not launch
       p->x_steps = xs;
@@ -1342,13 +1329,6 @@ int epb_exchange_init(epb_pool* p, int world, int rank, void* ipc_handle_out) {
   p->x_world = world;
   p->x_rank = rank;
   p->x_peer[rank] = p->x_base;
-  // kernels without the forwarding epilogue push; ENVPOOL_B200_EXCHANGE=push is the A/B switch
-  const char* mode = getenv("ENVPOOL_B200_EXCHANGE");
-  p->x_fused = p->fn.peer_epilogue && !(mode && strcmp(mode, "push") == 0);
-  // engine-captured chains: push on the side branch (default) or inside the step chain
-  // (ENVPOOL_B200_EXCHANGE_CHAIN=inline: the fused epilogue / the push kernel behind the step)
-  const char* cmode = getenv("ENVPOOL_B200_EXCHANGE_CHAIN");
-  p->x_side_push = !(cmode && strcmp(cmode, "inline") == 0);
   if (const char* to = getenv("ENVPOOL_B200_EXCHANGE_TIMEOUT_S")) {
     double sec = atof(to);
     if (sec > 0) p->x_timeout_ns = (long long)(sec * 1e9);
@@ -1435,7 +1415,7 @@ int exchange_step(epb_pool* p, const void* d_action, cudaStream_t s, int chain_k
   char* mine = p->x_base + p->x_mine(slot);
   int32_t* wire = reinterpret_cast<int32_t*>(mine + p->slab_bytes);
   const int force = d_action ? 0 : 1;
-  if (p->x_fused && !push_stream) {
+  if (p->fn.peer_epilogue && !push_stream) {
     int rc = launch_batch(p, d_action, nullptr, p->N, force, mine, s, p->x_view(slot), chain_k,
                           wire, next_action);
     if (rc != EPB_OK) return rc;

@@ -685,15 +685,6 @@ struct LaunchArgs {
 };
 typedef cudaError_t (*launch_fn)(const LaunchArgs&);
 
-// ENVPOOL_B200_PDL=0 turns the programmatic-dependent-launch attribute off (A/B switch).
-inline bool pdl_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("ENVPOOL_B200_PDL");
-    return !(e && e[0] == '0');
-  }();
-  return on;
-}
-
 // SMs of the current device (132 on an H100 SXM), read once per process: the GPUs of one node
 // are the same model.  Sizes grids and CTA caps; never changes what a kernel computes.
 inline int device_sm_count() {
@@ -708,13 +699,14 @@ inline int device_sm_count() {
 
 // CTA size of the single-step kernel: small batches are latency-bound and want many small
 // CTAs spread evenly over the SMs, large batches want fewer, fatter CTAs.
-// ENVPOOL_B200_STEP_BLOCK overrides (64 | 128 | 256).
+// ENVPOOL_B200_STEP_BLOCK=64 | 128 forces one of the two, so tests can run small crafted
+// batches through the 128-thread kernel.
 inline int step_block_for(int n) {
   static const int forced = [] {
     const char* e = getenv("ENVPOOL_B200_STEP_BLOCK");
     return e ? atoi(e) : 0;
   }();
-  if (forced == 64 || forced == 128 || forced == 256) return forced;
+  if (forced == 64 || forced == 128) return forced;
   return n <= device_sm_count() * 8 * 128 ? 64 : 128;
 }
 
@@ -731,15 +723,10 @@ cudaError_t launch_step_b(const LaunchArgs& a) {
   cfg.attrs = attr;
   // PDL pays off for direct launches (hides part of the launch latency of every step); inside
   // a captured graph the programmatic edges measured slower than plain kernel->kernel edges, so
-  // captures keep full serialisation (ENVPOOL_B200_PDL_GRAPH=1 for an A/B run).
+  // captures keep full serialisation.
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   cudaStreamIsCapturing(a.stream, &cap);
-  static const bool pdl_in_graph = [] {
-    const char* e = getenv("ENVPOOL_B200_PDL_GRAPH");
-    return e && e[0] == '1';
-  }();
-  cfg.numAttrs =
-      (pdl_enabled() && (cap == cudaStreamCaptureStatusNone || pdl_in_graph)) ? 1 : 0;
+  cfg.numAttrs = cap == cudaStreamCaptureStatusNone ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, step_kernel<Env, kB>, a.sv, a.ov,
                             static_cast<const typename Env::Act*>(a.action), a.env_ids, a.n,
                             a.force_reset, a.peers,
@@ -750,7 +737,6 @@ template <class Env>
 cudaError_t launch_step(const LaunchArgs& a) {
   switch (step_block_for(a.n)) {
     case 64: return launch_step_b<Env, 64>(a);
-    case 256: return launch_step_b<Env, 256>(a);
     default: return launch_step_b<Env, 128>(a);
   }
 }

@@ -19,11 +19,12 @@
 // copy) and the wire columns go into slot[t % D][rank] of every peer with 16-byte stores,
 // after which the step's sequence number is published in data_flag[rank] of every rank.
 // Producers of the peer stores:
-//   * fused (classic_control / toy_text): the step kernel's own epilogue -- each CTA forwards
-//     the rows it has just written (`peer_forward_rows`), so the transfer rides inside the
-//     step launch;
-//   * `push_kernel` (HalfCheetah, or ENVPOOL_B200_EXCHANGE=push): a copy kernel behind the
-//     step kernel (capi.cu).
+//   * fused: the step kernel's own epilogue -- each CTA forwards the rows it has just written
+//     (`peer_forward_rows`), so the transfer rides inside the step launch.  Direct exchanged
+//     steps and uncaptured chains of every thread-per-env kind;
+//   * `push_kernel`: a copy kernel of its own (capi.cu).  HalfCheetah's steps, behind the
+//     step kernel; and every kind's steps in captured chains, on branches beside the step
+//     chain (capi.cu `run_chain`).
 // Flow control.  D slots form a ring, so a rank may run up to D-1 steps ahead of the slowest
 // consumer: step t+1 computes and pushes while the data of step t is still in flight or being
 // consumed (the sender never waits for the transfer of the previous step).  Slot t % D may be

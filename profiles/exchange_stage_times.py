@@ -1,8 +1,8 @@
 """Stage times of ONE exchanged step, per rank, un-pipelined (run under torchrun on N GPUs):
 CUDA events on the pool's stream around  step(+push)  and  wait  of the direct API
 (epb_step_exchange_device / epb_exchange_wait), which serialises  step -> push -> wait  on one
-stream.  ENVPOOL_B200_EXCHANGE=push splits the first stage into the step kernel and the copy
-kernel (they are separate launches then; the sum is what the events see).  Prints one JSON line
+stream.  For HalfCheetah, which has no forwarding epilogue, the first stage is the step kernel
+and the copy kernel (separate launches; the sum is what the events see).  Prints one JSON line
 per rank: median microseconds of each stage and of the whole step."""
 import json
 import os
@@ -53,7 +53,6 @@ def main():
     b = np.array([e[k][1].elapsed_time(e[k][2]) for k in range(50, K)]) * 1e3
     tot = e[50][0].elapsed_time(e[K - 1][2]) * 1e3 / (K - 50)
     print(json.dumps({"rank": rank, "world": world, "task": task, "n": n,
-                      "mode": os.environ.get("ENVPOOL_B200_EXCHANGE", "fused"),
                       "step_push_us_med": round(float(np.median(a)), 2),
                       "wait_us_med": round(float(np.median(b)), 2),
                       "step_push_us_p10": round(float(np.percentile(a, 10)), 2),

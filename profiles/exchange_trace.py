@@ -44,7 +44,6 @@ def main():
     t0 = tr[tr > 0].min()
     rel = np.where(tr > 0, (tr - t0) / 1e3, -1.0)
     print(json.dumps({"rank": rank, "task": task, "n": n, "us_per_step": round(ms_ / K * 1e3, 2),
-                      "mode": os.environ.get("ENVPOOL_B200_EXCHANGE_CHAIN", "side"),
                       "depth": os.environ.get("ENVPOOL_B200_EXCHANGE_DEPTH", "4"),
                       "push_ctas": os.environ.get("ENVPOOL_B200_PUSH_CTAS", "default"),
                       "cols": ["push_start", "push_credit", "push_publish", "wait_start",

@@ -29,6 +29,7 @@ import numpy as np
 
 from helpers import (HC_DEFAULT, INT_TASKS, assert_batch_equal, assert_hc_env_algebra,
                      random_actions)
+from oracle.pgx_lib import ACTIONS as PGX_ACTIONS
 from test_gpu_parity import FLOAT_ATOL_F64
 
 
@@ -112,6 +113,25 @@ KINDS = {k.name: k for k in [
     Kind("HalfCheetah", "HalfCheetah", max_episode_steps=8),
 ]}
 CLASSIC = ["CartPole", "Pendulum", "Acrobot", "MountainCar", "MountainCarContinuous"]
+
+
+class PgxKind(Kind):
+    """A PGX game.  `oracle` returns None because the twins' comparison here reads a single-row
+    info:players.env_id; test_gpu_pgx.py holds the twins to the oracle instead."""
+
+    def actions(self, rng, shape):
+        a = rng.integers(-1, PGX_ACTIONS[self.task] + 1, size=shape)
+        return np.where(rng.random(shape) < 0.9,
+                        rng.integers(0, PGX_ACTIONS[self.task], size=shape), a).astype(np.int32)
+
+    def oracle(self, ids, seed, precision):
+        return None
+
+
+# (kind, precision) whose wire columns captured exchanged chains push through push_kernel:
+# every kind above, the classic kinds in f32 as well, and the two-player PGX games.
+PUSHED = ([(KINDS[k], "f64") for k in KINDS] + [(KINDS[k], "f32") for k in CLASSIC] +
+          [(PgxKind(g, g), "f64") for g in ("TicTacToe", "ConnectFour")])
 # bench.py's configurations (TASKS: registered limits and iopt, seed 0)
 BENCH_KINDS = {
     "CartPole": Kind("CartPole", "CartPole", max_episode_steps=500),

@@ -5,10 +5,10 @@ exchanged chains and the settings the engine reads once per process.  Run as
         python tests/exchange_matrix_check.py <group>
 
 with group one of depth<D> (ENVPOOL_B200_EXCHANGE_DEPTH=D), block<B> (ENVPOOL_B200_STEP_BLOCK=B),
-push<C> (ENVPOOL_B200_PUSH_CTAS=C) or bench.  The command starts one process per rank (W = 2, the
-same command with --rank r) on device 0; they meet in a gloo group and attach to each other's
-gather buffers through CUDA IPC, as the one-process-per-GPU deployment does (exchange_cases.py
-says why one process cannot play both ranks of an overlapped chain).  Each rank checks its own
+push<C> (ENVPOOL_B200_PUSH_CTAS=C), kinds or bench.  The command starts one process per rank
+(W = 2, the same command with --rank r) on device 0; they meet in a gloo group and attach to
+each other's gather buffers through CUDA IPC, as the one-process-per-GPU deployment does
+(exchange_cases.py says why one process cannot play both ranks of an overlapped chain).  Each rank checks its own
 gathered batch against all W twins after every call, rank 0 the twins against the oracle;
 prints `OK <group>` when both ranks finished."""
 import os
@@ -21,7 +21,7 @@ import time
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 sys.path.insert(0, HERE)
-from exchange_cases import BENCH_KINDS, KINDS, Ranks, set_env  # noqa: E402
+from exchange_cases import BENCH_KINDS, KINDS, PUSHED, Ranks  # noqa: E402
 
 WORLD = 2
 
@@ -35,24 +35,21 @@ def depth_group(D, rank):
     """Chains of lengths 1, D-1, D+1, 7, 2D, ... move the next chain through the slot phases;
     the (K, phase) keys outnumber the 8 cached graphs, so captures are evicted and redone."""
     for name in ("CartPole", "Acrobot", "Taxi", "HalfCheetah"):
-        for mode in ("side", "inline"):
-            set_env(EXCHANGE_CHAIN=mode)
-            with Ranks(KINDS[name], 1001, WORLD, rank=rank) as x:
-                x.attach()
-                assert x.depth == D, (x.depth, D)
-                x.reset()
-                keys = set()
-                for K in (1, D - 1, D + 1, 7, 2 * D, 3, 2, 5, 1, 4, 6):
-                    keys.add(x.chain(K, use_graph=True))
-                for K in (D + 1, 3):
-                    x.chain(K, use_graph=False)
-                x.timed(5, D + 2)
-                x.steps_direct(3)
-                for K in (1, D - 1, D + 1, 7, 2, 3):
-                    keys.add(x.chain(K, use_graph=True))
-                assert len({(K, phase) for K, _, phase in keys}) > 8, keys
-            say(rank, f"  depth {D} {name} {mode}: {x.steps} steps")
-    set_env(EXCHANGE_CHAIN=None)
+        with Ranks(KINDS[name], 1001, WORLD, rank=rank) as x:
+            x.attach()
+            assert x.depth == D, (x.depth, D)
+            x.reset()
+            keys = set()
+            for K in (1, D - 1, D + 1, 7, 2 * D, 3, 2, 5, 1, 4, 6):
+                keys.add(x.chain(K, use_graph=True))
+            for K in (D + 1, 3):
+                x.chain(K, use_graph=False)
+            x.timed(5, D + 2)
+            x.steps_direct(3)
+            for K in (1, D - 1, D + 1, 7, 2, 3):
+                keys.add(x.chain(K, use_graph=True))
+            assert len({(K, phase) for K, _, phase in keys}) > 8, keys
+        say(rank, f"  depth {D} {name}: {x.steps} steps")
 
 
 def block_group(B, rank):
@@ -69,8 +66,8 @@ def block_group(B, rank):
 
 
 def push_group(C, rank):
-    """push_kernel with C CTAs: tens of passes per thread over the wire columns."""
-    set_env(EXCHANGE="push")
+    """push_kernel with C CTAs: tens of passes per thread over the wire columns (every step of
+    HalfCheetah, CartPole's steps in captured chains)."""
     for name, n in (("HalfCheetah", 4097), ("CartPole", 65537)):
         with Ranks(KINDS[name], n, WORLD, rank=rank) as x:
             x.attach()
@@ -80,7 +77,19 @@ def push_group(C, rank):
             x.chain(3, use_graph=False)
             x.timed(4, 4)
         say(rank, f"  push {C} {name}: {x.steps} steps")
-    set_env(EXCHANGE=None)
+
+
+def kinds_group(rank):
+    """push_kernel on the wire columns of every kind: captured chains of D + 1 steps put each
+    step's pushes on a branch beside the step chain, 40 steps in all, so that envs reset
+    through the exchange.  Rank 0 prints one line per case."""
+    for kind, precision in PUSHED:
+        with Ranks(kind, 1001, WORLD, precision=precision, rank=rank) as x:
+            x.attach()
+            x.reset()
+            while x.steps < 40:
+                x.chain(x.depth + 1, use_graph=True)
+        say(rank, f"  kinds {kind.name}-{precision}: {x.steps} steps")
 
 
 # bench.py at --gpus 2: (kind, envs per rank, timed steps K, lead).  CartPole is the headline
@@ -132,6 +141,8 @@ def run_rank(group, rank, port):
         block_group(int(group[5:]), rank)
     elif group.startswith("push"):
         push_group(int(group[4:]), rank)
+    elif group == "kinds":
+        kinds_group(rank)
     elif group == "bench":
         bench_group(rank)
     else:

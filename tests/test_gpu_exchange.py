@@ -67,16 +67,14 @@ def test_two_ranks_one_device(task, kw, n_act):
         p.close()
 
 
-@pytest.mark.parametrize("task,chain_mode", [("CartPole", "side"), ("Catch", "side"),
-                                             ("CartPole", "inline")])
-def test_captured_exchange_chain_runs_ahead_of_the_waits(task, chain_mode):
+@pytest.mark.parametrize("task", ["CartPole", "Catch"], ids=lambda t: f"{t}-side")
+def test_captured_exchange_chain_runs_ahead_of_the_waits(task):
     """epb_step_exchange_many_device: K exchanged steps in one CUDA graph, the waits on a
     parallel branch, so step t+1..t+depth-2 compute and push while the batch of step t is
     still arriving (ring slots + credit / ack flags).  After every chain both ranks hold the
-    oracle's full batch; the un-captured chain gives the same bytes.  chain_mode: where the peer
-    stores are issued in the captured chain -- "side" (default): a copy kernel on the side
-    branch, so the step chain itself never waits for NVLink; "inline": the step kernel's fused
-    epilogue (ENVPOOL_B200_EXCHANGE_CHAIN).
+    oracle's full batch; the un-captured chain gives the same bytes.  The captured chain issues
+    the peer stores from a copy kernel on a side branch, so the step chain itself never waits
+    for NVLink.
 
     Runs in a subprocess (tests/exchange_chain_check.py) with CUDA_DEVICE_MAX_CONNECTIONS=32:
     two ranks played by ONE process on ONE device share that process's hardware launch queues,
@@ -90,7 +88,7 @@ def test_captured_exchange_chain_runs_ahead_of_the_waits(task, chain_mode):
 
     here = os.path.dirname(os.path.abspath(__file__))
     env = dict(os.environ, CUDA_DEVICE_MAX_CONNECTIONS="32",
-               ENVPOOL_B200_EXCHANGE_TIMEOUT_S="20", ENVPOOL_B200_EXCHANGE_CHAIN=chain_mode)
+               ENVPOOL_B200_EXCHANGE_TIMEOUT_S="20")
     out = subprocess.run([sys.executable, os.path.join(here, "exchange_chain_check.py"), task],
                          capture_output=True, text=True, timeout=600, env=env)
     assert out.returncode == 0, out.stdout[-3000:] + out.stderr[-3000:]

@@ -8,43 +8,39 @@ before any wait is enqueued.  Chains and timed chains overlap the ranks' steps, 
 by design, so they run with one process per rank, attached through CUDA IPC as in the
 one-process-per-GPU deployment (tests/exchange_matrix_check.py; exchange_cases.py says why),
 one group of processes per setting of the variables the engine reads once per process or at
-exchange_init."""
+exchange_init, and one for the pushes of every kind's captured chains."""
 import os
 import subprocess
 import sys
 
 import pytest
 
-from exchange_cases import CLASSIC, KINDS, Ranks
+from exchange_cases import CLASSIC, KINDS, PUSHED, Ranks
 
 pytestmark = pytest.mark.gpu
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
-# (kind, precision, mode): every kind with the fused epilogue (its default) and with
-# ENVPOOL_B200_EXCHANGE=push; the classic kinds in f32 as well.  HalfCheetah has no fused
-# epilogue, so its default is the push kernel: one row.
-DIRECT = ([(k, "f64", m) for k in KINDS if k != "HalfCheetah" for m in ("fused", "push")] +
-          [("HalfCheetah", "f64", "push")] +
-          [(k, "f32", m) for k in CLASSIC for m in ("fused", "push")])
+# (kind, precision): every kind, the classic kinds in f32 as well.  The id names what forwards
+# the wire columns of a direct exchanged step: the step kernel's fused epilogue, or push_kernel
+# for HalfCheetah, which has none.
+DIRECT = [(k, "f64") for k in KINDS] + [(k, "f32") for k in CLASSIC]
 
 
 @pytest.fixture
 def exchange_env(monkeypatch):
-    """Leave no ENVPOOL_B200_EXCHANGE* setting behind for the next test."""
-    for k in ("EXCHANGE", "EXCHANGE_DEPTH", "EXCHANGE_CHAIN"):
-        monkeypatch.delenv("ENVPOOL_B200_" + k, raising=False)
+    """Leave no ENVPOOL_B200_EXCHANGE_DEPTH setting behind for the next test."""
+    monkeypatch.delenv("ENVPOOL_B200_EXCHANGE_DEPTH", raising=False)
     return monkeypatch
 
 
-@pytest.mark.parametrize("kind,precision,mode", DIRECT,
-                         ids=[f"{k}-{p}-{m}" for k, p, m in DIRECT])
-def test_direct_exchanged_steps_every_kind(capi, exchange_env, kind, precision, mode):
+@pytest.mark.parametrize("kind,precision", DIRECT,
+                         ids=[f"{k}-{p}-{'push' if k == 'HalfCheetah' else 'fused'}"
+                              for k, p in DIRECT])
+def test_direct_exchanged_steps_every_kind(capi, exchange_env, kind, precision):
     """W = 2, n = 1001 per rank (not a multiple of 4, 16 or 64: the wait kernel's tail quad,
-    partial 16-byte units in push_kernel and peer_forward_rows, a partial last CTA), 40 steps
+    partial 16-byte units in peer_forward_rows and push_kernel, a partial last CTA), 40 steps
     with episodes short enough that envs reset through the exchange."""
-    if mode == "push":
-        exchange_env.setenv("ENVPOOL_B200_EXCHANGE", "push")
     with Ranks(KINDS[kind], 1001, 2, precision=precision) as x:
         x.attach()
         x.reset()
@@ -85,14 +81,18 @@ def test_128_thread_step_kernel_forwards_its_rows(capi, exchange_env):
         x.steps_direct(12)
 
 
-def _run_group(group, **env):
+def _group(group, **env):
     full = dict(os.environ, CUDA_DEVICE_MAX_CONNECTIONS="32",
                 ENVPOOL_B200_EXCHANGE_TIMEOUT_S="20")
-    for k in ("EXCHANGE", "EXCHANGE_DEPTH", "EXCHANGE_CHAIN", "STEP_BLOCK", "PUSH_CTAS"):
+    for k in ("EXCHANGE_DEPTH", "STEP_BLOCK", "PUSH_CTAS"):
         full.pop("ENVPOOL_B200_" + k, None)
     full.update({"ENVPOOL_B200_" + k: str(v) for k, v in env.items()})
-    out = subprocess.run([sys.executable, os.path.join(HERE, "exchange_matrix_check.py"), group],
-                         capture_output=True, text=True, timeout=900, env=full)
+    return subprocess.run([sys.executable, os.path.join(HERE, "exchange_matrix_check.py"), group],
+                          capture_output=True, text=True, timeout=900, env=full)
+
+
+def _run_group(group, **env):
+    out = _group(group, **env)
     assert out.returncode == 0, out.stdout[-3000:] + out.stderr[-3000:]
     assert f"OK {group}" in out.stdout, out.stdout[-3000:]
 
@@ -114,17 +114,17 @@ def test_ring_depths_direct_steps(capi, exchange_env, kind, depth):
 @pytest.mark.parametrize("depth", [2, 3, 4, 5, 8])
 def test_chains_at_every_ring_depth_and_slot_phase(depth):
     """ENVPOOL_B200_EXCHANGE_DEPTH = 2, 3, 4 (the default), 5, 8 for CartPole, Acrobot, Taxi and
-    HalfCheetah: captured chains in `side` and `inline` mode and uncaptured chains of lengths
+    HalfCheetah: captured and uncaptured chains of lengths
     1, D-1, D+1, 7, 2D, ... that start the next chain at every slot phase, more (K, phase) graph
     keys than the cache holds (evictions and recaptures), then a timed exchanged chain, direct
     exchanged steps and chains again."""
     _run_group(f"depth{depth}", EXCHANGE_DEPTH=depth)
 
 
-@pytest.mark.parametrize("block", [128, 256])
+@pytest.mark.parametrize("block", [128])
 def test_step_kernel_cta_sizes(block):
-    """ENVPOOL_B200_STEP_BLOCK = 128 / 256 (read once per process): the fused epilogue of the
-    wider step kernels, for rows of 12 (Pendulum, Blackjack obs), 24 + 8 (Acrobot) and 100
+    """ENVPOOL_B200_STEP_BLOCK = 128 (read once per process): the fused epilogue of the
+    wider step kernel, for rows of 12 (Pendulum, Blackjack obs), 24 + 8 (Acrobot) and 100
     bytes (Minesweeper's action mask), none a multiple of 16."""
     _run_group(f"block{block}", STEP_BLOCK=block)
 
@@ -132,8 +132,24 @@ def test_step_kernel_cta_sizes(block):
 @pytest.mark.parametrize("ctas", [1, 3])
 def test_push_kernel_grids(ctas):
     """ENVPOOL_B200_PUSH_CTAS = 1 / 3 (read once per process): every push thread makes many
-    passes over the wire columns (HalfCheetah, and CartPole with ENVPOOL_B200_EXCHANGE=push)."""
+    passes over the wire columns (HalfCheetah, and CartPole's captured chains)."""
     _run_group(f"push{ctas}", PUSH_CTAS=ctas)
+
+
+@pytest.fixture(scope="module")
+def kinds_group():
+    """The `kinds` group runs every case of the test below in one pair of processes."""
+    return _group("kinds")
+
+
+@pytest.mark.parametrize("kind,precision", PUSHED, ids=[f"{k.name}-{p}" for k, p in PUSHED])
+def test_push_kernel_every_kind(kinds_group, kind, precision):
+    """push_kernel on every kind's wire columns: captured exchanged chains of D + 1 steps put
+    the pushes on branches beside the step chain, 40 steps with envs resetting through the
+    exchange (direct steps forward through the fused epilogue instead)."""
+    out = kinds_group
+    assert out.returncode == 0 and f"kinds {kind.name}-{precision}: " in out.stdout, \
+        out.stdout[-3000:] + out.stderr[-3000:]
 
 
 def test_benchmark_shapes_through_the_timed_exchange_chain():

@@ -1,10 +1,6 @@
 """GPU: Jumanji Minesweeper-v0 on the sm_90a kernel (envpool_b200/csrc/jumanji.cu), bit for bit
 against the oracle (oracle/ms_oracle.c), the reference's own thread pool (oracle/_ref, when the
 build made it) and the fixtures recorded from it, through every entry point of the engine."""
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
@@ -361,35 +357,6 @@ def test_large_pool_runs_the_128_thread_kernel(capi):
         lo.step_device(d[:H].contiguous())
         hi.step_device(d[H:].contiguous())
         wf, wl = first.step(a[:P]), last.step(a[N - P:])
-
-
-_BLOCK_256 = """
-import numpy as np
-from envpool_b200 import _capi
-from test_gpu_minesweeper import actions, make_pool, meta_for, eq
-from test_minesweeper import oracle_for
-_capi.load_library()
-for config in ("default", "replay"):
-    meta = meta_for(config, 5000, 83)
-    pool, orc = make_pool(_capi, meta), oracle_for(meta)
-    rng = np.random.default_rng(23)
-    eq(pool.reset(), orc.reset(), "reset")
-    for t in range(120):
-        a = actions(rng, 5000)
-        eq(pool.step(a), orc.step(a), f"{config} t={t}")
-print("BLOCK256 OK")
-"""
-
-
-def test_256_thread_step_kernel_in_a_subprocess(capi):
-    """ENVPOOL_B200_STEP_BLOCK=256 is read once per process: a fresh interpreter steps a pool
-    on the 256-thread kernel (13 KB of staged boards per CTA) against the oracle."""
-    here = os.path.dirname(os.path.abspath(__file__))
-    env = dict(os.environ, ENVPOOL_B200_STEP_BLOCK="256",
-               PYTHONPATH=os.pathsep.join([os.path.dirname(here), here]))
-    r = subprocess.run([sys.executable, "-s", "-c", _BLOCK_256], env=env, cwd=here,
-                       capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "BLOCK256 OK" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
 
 
 def test_two_ranks_one_device(capi):

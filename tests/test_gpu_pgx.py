@@ -3,8 +3,8 @@ the C restatement (oracle/pgx_oracle.c), the reference's own thread pool (oracle
 build() made it) and the fixtures recorded from it (tests/golden/pgx/), through every entry
 point: the host path (sync, async, permuted and partial batches), the pybind `_send` with
 explicit players.env_id rows, make_gymnasium / make_dm, step_device, the step chains (graph and
-direct), the timed chain, the fused rollout, snapshots, the 64-, 128- and 256-thread step kernels
-and the peer exchange."""
+direct), the timed chain, the fused rollout, snapshots, the 64- and 128-thread step kernels and
+the peer exchange."""
 import glob
 import json
 import os
@@ -338,10 +338,10 @@ print("ok")
 """
 
 
-@pytest.mark.parametrize("block", [64, 256])
+@pytest.mark.parametrize("block", [64])
 def test_forced_step_kernel_block(block):
-    """ENVPOOL_B200_STEP_BLOCK is read once per process: the 64- and 256-thread step kernels run
-    in a subprocess of their own, at batch sizes that leave a partial last CTA."""
+    """ENVPOOL_B200_STEP_BLOCK is read once per process: the 64-thread step kernel runs in a
+    subprocess of its own, at batch sizes that leave a partial last CTA."""
     root = os.path.dirname(HERE)
     env = dict(os.environ, ENVPOOL_B200_STEP_BLOCK=str(block))
     r = subprocess.run([sys.executable, "-c", _BLOCK_BODY.format(root=root, tests=HERE)],
@@ -350,55 +350,31 @@ def test_forced_step_kernel_block(block):
 
 
 # ---------------------------------------------------------------------------- peer exchange
-from exchange_cases import Kind, Ranks  # noqa: E402
+from exchange_cases import PgxKind, Ranks  # noqa: E402
 
 
-class PgxKind(Kind):
-    """The exchange tests' view of a PGX game.  The exchange is held byte for byte to the
-    un-exchanged twins; `oracle` returns None because exchange_cases compares the twins with a
-    single-row info:players.env_id, and the twins are held to the oracle below instead."""
-
-    def pool(self, n, offset, seed, precision="f64"):
-        from envpool_b200 import _capi
-
-        return _capi.CPool(self.task, n, seed=seed, env_id_offset=offset, precision=precision)
-
-    def actions(self, rng, shape):
-        a = rng.integers(-1, ACTIONS[self.task] + 1, size=shape)
-        return np.where(rng.random(shape) < 0.9, rng.integers(0, ACTIONS[self.task], size=shape),
-                        a).astype(np.int32)
-
-    def oracle(self, ids, seed, precision):
-        return None
-
-
-@pytest.mark.parametrize("game", GAMES)
-@pytest.mark.parametrize("mode", ["fused", "push"])
-def test_exchange(game, mode):
+@pytest.mark.parametrize("game", GAMES, ids=lambda g: f"fused-{g}")
+def test_exchange(game):
+    """Direct exchanged steps (the step kernel's fused epilogue forwards both player rows) byte
+    for byte against the un-exchanged twins, and the twins against the oracle."""
     import torch
 
-    from exchange_cases import set_env
-
-    set_env(EXCHANGE=None if mode == "fused" else "push")
-    try:
-        n, W = 1001, 2
-        with Ranks(PgxKind(game, game), n, W) as x:
-            x.attach()
-            x.reset()
-            x.steps_direct(20)
-            # the twins against the oracle: global env g of rank r has seed + g
-            orc = PgxOracle(game, W * n, seed=x.seed, env_seed=np.arange(W * n) + x.seed)
-            orc.reset()
-            for t in range(20):
-                want = orc.step(x.acts[t % x.T])
-            got = {}
-            for k in x.twins[0].keys:
-                got[k.name] = np.concatenate([tw.outputs_torch()[k.name].cpu().numpy()
-                                              for tw in x.twins])
-            assert_same(got, want, f"{game} exchanged twins vs oracle")
-            torch.cuda.synchronize()
-    finally:
-        set_env(EXCHANGE=None)
+    n, W = 1001, 2
+    with Ranks(PgxKind(game, game), n, W) as x:
+        x.attach()
+        x.reset()
+        x.steps_direct(20)
+        # the twins against the oracle: global env g of rank r has seed + g
+        orc = PgxOracle(game, W * n, seed=x.seed, env_seed=np.arange(W * n) + x.seed)
+        orc.reset()
+        for t in range(20):
+            want = orc.step(x.acts[t % x.T])
+        got = {}
+        for k in x.twins[0].keys:
+            got[k.name] = np.concatenate([tw.outputs_torch()[k.name].cpu().numpy()
+                                          for tw in x.twins])
+        assert_same(got, want, f"{game} exchanged twins vs oracle")
+        torch.cuda.synchronize()
 
 
 # ---------------------------------------------------------------------------- pool layouts

@@ -1,7 +1,7 @@
 """GPU: the toy_text family (envpool_b200/csrc/toytext.cu) bit for bit against the oracle on
 every reachable state and action, in every compiled kernel and through every entry point.
 
-Each env is instantiated into four kernels -- step_kernel<Env, 64 / 128 / 256> and
+Each env is instantiated into three kernels -- step_kernel<Env, 64 / 128> and
 rollout_kernel<Env> -- that ptxas compiles one by one, so a miscompile can sit in one of them
 alone (toytext.cu's CliffWalking note records one).  The crafted pools of toy_text_cases.py
 (every reachable state x every action, mt19937 tables forced onto each draw's boundaries,
@@ -153,10 +153,10 @@ print("BLOCK%s OK" % sys.argv[1])
 """
 
 
-@pytest.mark.parametrize("block", [128, 256])
+@pytest.mark.parametrize("block", [128])
 def test_crafted_states_on_the_wide_step_kernels_in_a_subprocess(capi, block):
     """ENVPOOL_B200_STEP_BLOCK is read once per process: a fresh interpreter steps every
-    crafted pool on the 128- or 256-thread step kernel against the oracle."""
+    crafted pool on the 128-thread step kernel against the oracle."""
     here = os.path.dirname(os.path.abspath(__file__))
     env = dict(os.environ, ENVPOOL_B200_STEP_BLOCK=str(block),
                PYTHONPATH=os.pathsep.join([os.path.dirname(here), here]))
