@@ -301,9 +301,9 @@ int get_event(epb_pool* p, cudaEvent_t* ev) {
   return EPB_OK;
 }
 
-// Copy the wire columns of the local slice to every peer, then publish: behind the step for
-// kinds without the forwarding epilogue (HalfCheetah), and on the push branches of captured
-// chains for every kind.  Column k is ceil(n * row_bytes / 16) 16-byte units (the 256-byte
+// Copy the wire columns of the local slice to every peer, then publish: behind the step on its
+// own stream for direct steps and uncaptured chains, and on the push branches of captured
+// chains.  Column k is ceil(n * row_bytes / 16) 16-byte units (the 256-byte
 // column padding absorbs the tail).
 __global__ void __launch_bounds__(256)
 push_kernel(const PeerView* __restrict__ pv, int n) {
@@ -536,9 +536,8 @@ int launch_refill(epb_pool* p, cudaStream_t stream) {
 // refill itself (host path: behind the D2H copy; engine-captured chains: on a parallel graph
 // branch every refill_every steps, run_chain).
 int launch_batch(epb_pool* p, const void* d_action, const int32_t* d_ids, int n,
-                 int force_reset, char* d_slab, cudaStream_t stream,
-                 const PeerView* peers = nullptr, int chain_k = -1, int32_t* wire = nullptr,
-                 const void* next_action = nullptr) {
+                 int force_reset, char* d_slab, cudaStream_t stream, int chain_k = -1,
+                 int32_t* wire = nullptr, const void* next_action = nullptr) {
   p->d_last = d_slab;
   p->started = true;
   LaunchArgs a = launch_args(p, stream);
@@ -548,7 +547,6 @@ int launch_batch(epb_pool* p, const void* d_action, const int32_t* d_ids, int n,
   a.env_ids = d_ids;
   a.n = n;
   a.force_reset = force_reset;
-  a.peers = peers;
   a.next_action = next_action;
   EPB_CUDA(p->fn.step(a));
   ++p->launches;
@@ -611,8 +609,7 @@ int host_submit(epb_pool* p, const void* action, const int32_t* env_ids, int n,
   EPB_CUDA(cudaEventRecord(p->h_stage_ev[f], p->stream));
   // the step kernel alone; the refill of the records it consumed goes BEHIND the D2H copy
   // (the caller waits for the copy, not for the refill)
-  int rc = launch_batch(p, p->d_action, d_ids, n, force_reset, p->d_slab, p->stream, nullptr,
-                        -2);
+  int rc = launch_batch(p, p->d_action, d_ids, n, force_reset, p->d_slab, p->stream, -2);
   if (rc != EPB_OK) return rc;
   void* slab = nullptr;
   bool ids_ok = false;
@@ -1150,7 +1147,7 @@ int run_chain(epb_pool* p, cudaStream_t st, const ChainKey& c, bool fork, cudaEv
         //   waits     wait_derive(k) after push(k) and wait_derive(k-1)
         // A kernel that stores to a peer cannot complete -- and its successor on the same stream
         // cannot start -- before those stores have drained over NVLink, which takes several
-        // times the payload's link time, whether it is the fused epilogue or a copy kernel.
+        // times the payload's link time.
         // Round trips cannot be shortened, so they are overlapped.
         if (k >= D) EPB_CUDA(cudaStreamWaitEvent(st, p->x_ev_push[(k - D) % D], 0));
         cudaStream_t ps = p->x_push[k % 3];
@@ -1168,8 +1165,7 @@ int run_chain(epb_pool* p, cudaStream_t st, const ChainKey& c, bool fork, cudaEv
         if (rc != EPB_OK) return rc;
       }
     } else {
-      rc = launch_batch(p, a, nullptr, p->N, 0, p->d_slab, st, nullptr, rec ? -2 : -1, nullptr,
-                        nx);
+      rc = launch_batch(p, a, nullptr, p->N, 0, p->d_slab, st, rec ? -2 : -1, nullptr, nx);
       if (rc != EPB_OK) return rc;
     }
     if (rec && ((k % R) == R - 1 || k == c.K - 1)) {
@@ -1400,7 +1396,8 @@ int epb_exchange_attach_ipc(epb_pool* p, const void* ipc_handles) {
 namespace {
 
 // One exchanged step on `s`: the step kernel writes slot[t % D][rank] of the local allocation,
-// checks the credit (slot t % D released everywhere), forwards its wire columns, publishes.
+// then push_kernel -- on `push_stream` if given, else on `s` -- checks the credit (slot t % D
+// released everywhere), forwards the wire columns and publishes.
 int exchange_step(epb_pool* p, const void* d_action, cudaStream_t s, int chain_k,
                   const void* next_action, cudaStream_t push_stream, cudaEvent_t step_done) {
   const int D = p->x_depth;
@@ -1415,38 +1412,31 @@ int exchange_step(epb_pool* p, const void* d_action, cudaStream_t s, int chain_k
   char* mine = p->x_base + p->x_mine(slot);
   int32_t* wire = reinterpret_cast<int32_t*>(mine + p->slab_bytes);
   const int force = d_action ? 0 : 1;
-  if (p->fn.peer_epilogue && !push_stream) {
-    int rc = launch_batch(p, d_action, nullptr, p->N, force, mine, s, p->x_view(slot), chain_k,
-                          wire, next_action);
-    if (rc != EPB_OK) return rc;
-  } else {
-    int rc = launch_batch(p, d_action, nullptr, p->N, force, mine, s, nullptr, chain_k, wire,
-                          next_action);
-    if (rc != EPB_OK) return rc;
-    if (push_stream) {  // the copy kernel goes on the caller's side branch, behind this step
-      EPB_CUDA(cudaEventRecord(step_done, s));
-      EPB_CUDA(cudaStreamWaitEvent(push_stream, step_done, 0));
-      s = push_stream;
-    }
-    // CTAs of the copy kernel: eight 16-byte units per thread (two passes of four), at most 8
-    // CTAs per SM.  Every CTA ends in a system-scope fence, so fewer, fuller CTAs make the
-    // fence phase cheaper.  ENVPOOL_B200_PUSH_CTAS overrides.
-    static const int64_t cta_cap = [] {
-      const char* e = getenv("ENVPOOL_B200_PUSH_CTAS");
-      const int v = e ? atoi(e) : 0;
-      return (int64_t)(v > 0 ? v : device_sm_count() * 8);
-    }();
-    // reward + the packed word
-    int64_t n16 = ((int64_t)p->N * p->keys[4].row_bytes + 15) / 16 + ((int64_t)p->N * 4 + 15) / 16;
-    for (size_t k = 8; k < p->keys.size(); ++k)
-      n16 += ((int64_t)p->N * p->keys[k].row_bytes + 15) / 16;
-    int64_t blocks = (n16 + 2047) / 2048;
-    if (blocks > cta_cap) blocks = cta_cap;
-    if (blocks < 1) blocks = 1;
-    push_kernel<<<(unsigned)blocks, 256, 0, s>>>(p->x_view(slot), p->N);
-    EPB_CUDA(cudaGetLastError());
-    ++p->launches;
+  int rc = launch_batch(p, d_action, nullptr, p->N, force, mine, s, chain_k, wire, next_action);
+  if (rc != EPB_OK) return rc;
+  if (push_stream) {  // the copy kernel goes on the caller's side branch, behind this step
+    EPB_CUDA(cudaEventRecord(step_done, s));
+    EPB_CUDA(cudaStreamWaitEvent(push_stream, step_done, 0));
+    s = push_stream;
   }
+  // CTAs of the copy kernel: eight 16-byte units per thread (two passes of four), at most 8
+  // CTAs per SM.  Every CTA ends in a system-scope fence, so fewer, fuller CTAs make the
+  // fence phase cheaper.  ENVPOOL_B200_PUSH_CTAS overrides.
+  static const int64_t cta_cap = [] {
+    const char* e = getenv("ENVPOOL_B200_PUSH_CTAS");
+    const int v = e ? atoi(e) : 0;
+    return (int64_t)(v > 0 ? v : device_sm_count() * 8);
+  }();
+  // reward + the packed word
+  int64_t n16 = ((int64_t)p->N * p->keys[4].row_bytes + 15) / 16 + ((int64_t)p->N * 4 + 15) / 16;
+  for (size_t k = 8; k < p->keys.size(); ++k)
+    n16 += ((int64_t)p->N * p->keys[k].row_bytes + 15) / 16;
+  int64_t blocks = (n16 + 2047) / 2048;
+  if (blocks > cta_cap) blocks = cta_cap;
+  if (blocks < 1) blocks = 1;
+  push_kernel<<<(unsigned)blocks, 256, 0, s>>>(p->x_view(slot), p->N);
+  EPB_CUDA(cudaGetLastError());
+  ++p->launches;
   ++p->x_steps;
   return EPB_OK;
 }

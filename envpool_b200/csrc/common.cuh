@@ -492,7 +492,6 @@ template <class Env, int kB = kBlock>
 __global__ void __launch_bounds__(kB)
 step_kernel(StateView sv, OutView ov, const typename Env::Act* __restrict__ action,
             const int32_t* __restrict__ env_ids, int n, int force_reset,
-            const PeerView* __restrict__ peers,
             const typename Env::Act* __restrict__ next_action) {
   int row = blockIdx.x * kB + threadIdx.x;
   bool active = row < n;
@@ -541,8 +540,6 @@ step_kernel(StateView sv, OutView ov, const typename Env::Act* __restrict__ acti
   } else if (active) {
     Env::write_obs(sv, ov, row, s, so);
   }
-  // sharded pools: forward this CTA's output rows to every peer GPU (exchange.cuh)
-  if (peers) peer_forward_rows<kB>(peers, (int64_t)blockIdx.x * kB, n);
 }
 
 // Refills every env's record ring to rec_q valid records (draws rec_q - (rprod - rcons) new
@@ -679,7 +676,6 @@ struct LaunchArgs {
   int force_reset;
   int T;  // rollout only
   cudaStream_t stream;
-  const PeerView* peers;  // device pointer; non-NULL = fused peer exchange epilogue
   const void* next_action;  // step chains: action row of the following step (L2 prefetch)
   const void* params;       // the pool's family parameters (KindDesc::setup; HalfCheetah only)
 };
@@ -729,8 +725,7 @@ cudaError_t launch_step_b(const LaunchArgs& a) {
   cfg.numAttrs = cap == cudaStreamCaptureStatusNone ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, step_kernel<Env, kB>, a.sv, a.ov,
                             static_cast<const typename Env::Act*>(a.action), a.env_ids, a.n,
-                            a.force_reset, a.peers,
-                            static_cast<const typename Env::Act*>(a.next_action));
+                            a.force_reset, static_cast<const typename Env::Act*>(a.next_action));
 }
 
 template <class Env>
@@ -770,7 +765,6 @@ struct EnvKey {
 struct KindLaunch {
   launch_fn step, rollout;
   launch_fn refill;      // non-NULL: resets come from the reset-ahead records (StateView::rec)
-  bool peer_epilogue;    // the step kernel forwards its rows to the peers (exchange.cuh)
   // added to bytes_per_env_step's count of action, state and columns: per-step RNG traffic,
   // less any state words a step does not touch
   int extra_step_bytes;
@@ -805,7 +799,7 @@ template <class Env>
 KindLaunch kind_launch(int extra_step_bytes = 0) {
   launch_fn refill = nullptr;
   if constexpr (UsesRec<Env>::value) refill = launch_refill<Env>;
-  return {launch_step<Env>, launch_rollout<Env>, refill, true, extra_step_bytes};
+  return {launch_step<Env>, launch_rollout<Env>, refill, extra_step_bytes};
 }
 // the launch of a kind whose kernels depend on neither precision nor iopt
 template <class Env, int kExtraStepBytes = 0>

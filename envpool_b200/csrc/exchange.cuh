@@ -18,13 +18,10 @@
 // A step writes its slab straight into slot[t % D][rank] of the LOCAL allocation (no staging
 // copy) and the wire columns go into slot[t % D][rank] of every peer with 16-byte stores,
 // after which the step's sequence number is published in data_flag[rank] of every rank.
-// Producers of the peer stores:
-//   * fused: the step kernel's own epilogue -- each CTA forwards the rows it has just written
-//     (`peer_forward_rows`), so the transfer rides inside the step launch.  Direct exchanged
-//     steps and uncaptured chains of every thread-per-env kind;
-//   * `push_kernel`: a copy kernel of its own (capi.cu).  HalfCheetah's steps, behind the
-//     step kernel; and every kind's steps in captured chains, on branches beside the step
-//     chain (capi.cu `run_chain`).
+// The one producer of the peer stores is `push_kernel` (capi.cu), a copy kernel of its own
+// behind the step kernel: on the step's stream for direct steps and uncaptured chains, on
+// branches beside the step chain in captured chains (capi.cu `run_chain`).  The step kernels
+// know nothing of the exchange beyond the packed wire column they write.
 // Flow control.  D slots form a ring, so a rank may run up to D-1 steps ahead of the slowest
 // consumer: step t+1 computes and pushes while the data of step t is still in flight or being
 // consumed (the sender never waits for the transfer of the previous step).  Slot t % D may be
@@ -174,71 +171,6 @@ __device__ __forceinline__ void peer_publish(const PeerView* __restrict__ pv) {
       for (int g = 0; g < world; ++g) st_relaxed_sys(pv->flag[g], t + 1);
     }
   }
-}
-
-// Fused epilogue of the step kernels: the CTA forwards the wire columns of the output rows
-// [row0, row0 + kB) it has just written into its local slice to every peer, then publishes.
-// The rows of all wire columns are treated as one list of 16-byte units (column k contributes
-// ceil(rows * row_bytes / 16) of them); each thread loads up to four units before it issues
-// any peer store, so the L2 read latency is paid once, not once per column.  Requires the
-// identity row<->env mapping (sync step of all envs) and kB % 16 == 0, so that every
-// per-column chunk starts 16-byte aligned; the tail CTA may copy up to 15 bytes past its
-// last row, which stays inside the column's 256-byte padding.
-template <int kB>
-__device__ __forceinline__ void peer_forward_rows(const PeerView* __restrict__ pv, int64_t row0,
-                                                  int n) {
-  static_assert(kB % 16 == 0, "CTA rows must keep 1-byte columns 16-byte aligned");
-  __shared__ int s_first[kMaxCols + 1];   // first unit of column k in this CTA's unit list
-  __shared__ int64_t s_off[kMaxCols];     // slice byte offset of this CTA's rows in column k
-  __shared__ char* s_peer[kMaxPeers];
-  const int64_t left = (int64_t)n - row0;
-  const int rows = left < kB ? (int)left : kB;
-  const int world = pv->world, rank = pv->rank, ncols = pv->ncols;
-  const int tid = threadIdx.x;
-  if (tid < ncols) {
-    const int rb = pv->col_rb[tid];
-    s_first[tid + 1] = (rows * rb + 15) >> 4;
-    s_off[tid] = pv->col_off[tid] + row0 * rb;
-  }
-  if (tid < world) s_peer[tid] = pv->slice[tid];
-  peer_credit(pv);  // every peer has released the slot these rows go into
-  __syncthreads();  // tables ready; all rows of this CTA are written (by this CTA)
-  if (tid == 0) {
-    int acc = 0;
-    s_first[0] = 0;
-    for (int k = 0; k < ncols; ++k) {
-      acc += s_first[k + 1];
-      s_first[k + 1] = acc;
-    }
-  }
-  __syncthreads();
-  const int total = s_first[ncols];
-  const char* local = s_peer[rank];
-  constexpr int kU = 4;
-  for (int u0 = tid; u0 < total; u0 += kU * kB) {
-    uint4 v[kU];
-    int64_t off[kU];
-#pragma unroll
-    for (int j = 0; j < kU; ++j) {
-      const int u = u0 + j * kB;
-      off[j] = -1;
-      if (u < total) {
-        int k = 0;
-        while (u >= s_first[k + 1]) ++k;
-        off[j] = s_off[k] + 16 * (int64_t)(u - s_first[k]);
-        v[j] = *reinterpret_cast<const uint4*>(local + off[j]);
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < kU; ++j) {
-      if (off[j] >= 0) {
-#pragma unroll 1
-        for (int g = 0; g < world; ++g)
-          if (g != rank) *reinterpret_cast<uint4*>(s_peer[g] + off[j]) = v[j];
-      }
-    }
-  }
-  peer_publish(pv);
 }
 
 }  // namespace epb

@@ -7,8 +7,8 @@ do not depend on G.  The one exchange step of the path is an all-gather of the o
 columns, which reassembles the full `[num_envs, ...]` batch on every rank.  Two transports:
 
 * the engine's own peer exchange (csrc/exchange.cuh): the step writes into this rank's slice
-  of a ring of gather slots that every peer maps through CUDA IPC, its epilogue stores the
-  columns a peer cannot derive (env keys, reward, one packed word) into all peers over
+  of a ring of gather slots that every peer maps through CUDA IPC, a copy kernel behind it stores
+  the columns a peer cannot derive (env keys, reward, one packed word) into all peers over
   NVLink and raises sequence flags; the receiver re-expands the rest --
   `enable_peer_exchange()`, `reset_exchange()`, `step_exchange(actions)`;
 * `torch.distributed` all-gather (NCCL on GPUs; gloo on CPU tensors in the host-logic

@@ -1,9 +1,8 @@
 """Stage times of ONE exchanged step, per rank, un-pipelined (run under torchrun on N GPUs):
 CUDA events on the pool's stream around  step(+push)  and  wait  of the direct API
 (epb_step_exchange_device / epb_exchange_wait), which serialises  step -> push -> wait  on one
-stream.  For HalfCheetah, which has no forwarding epilogue, the first stage is the step kernel
-and the copy kernel (separate launches; the sum is what the events see).  Prints one JSON line
-per rank: median microseconds of each stage and of the whole step."""
+stream.  The first stage is the step kernel and the copy kernel that forwards its rows
+(separate launches; the sum is what the events see).  Prints one JSON line per rank: median microseconds of each stage and of the whole step."""
 import json
 import os
 import sys

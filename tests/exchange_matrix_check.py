@@ -53,7 +53,8 @@ def depth_group(D, rank):
 
 
 def block_group(B, rank):
-    """The fused epilogue of the B-thread step kernel (every pool here runs it, twins too)."""
+    """The B-thread step kernel writing its ring slot before push_kernel forwards it (every
+    pool here runs that kernel, twins too)."""
     for name in ("Pendulum", "Acrobot", "Blackjack", "Minesweeper"):
         with Ranks(KINDS[name], 1001, WORLD, rank=rank) as x:
             x.attach()

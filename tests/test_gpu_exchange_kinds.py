@@ -21,9 +21,8 @@ pytestmark = pytest.mark.gpu
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
-# (kind, precision): every kind, the classic kinds in f32 as well.  The id names what forwards
-# the wire columns of a direct exchanged step: the step kernel's fused epilogue, or push_kernel
-# for HalfCheetah, which has none.
+# (kind, precision): every kind, the classic kinds in f32 as well.  push_kernel forwards the
+# wire columns of every direct exchanged step, behind the step kernel on the same stream.
 DIRECT = [(k, "f64") for k in KINDS] + [(k, "f32") for k in CLASSIC]
 
 
@@ -34,12 +33,10 @@ def exchange_env(monkeypatch):
     return monkeypatch
 
 
-@pytest.mark.parametrize("kind,precision", DIRECT,
-                         ids=[f"{k}-{p}-{'push' if k == 'HalfCheetah' else 'fused'}"
-                              for k, p in DIRECT])
+@pytest.mark.parametrize("kind,precision", DIRECT, ids=[f"{k}-{p}" for k, p in DIRECT])
 def test_direct_exchanged_steps_every_kind(capi, exchange_env, kind, precision):
     """W = 2, n = 1001 per rank (not a multiple of 4, 16 or 64: the wait kernel's tail quad,
-    partial 16-byte units in peer_forward_rows and push_kernel, a partial last CTA), 40 steps
+    partial 16-byte units in push_kernel, a partial last step CTA), 40 steps
     with episodes short enough that envs reset through the exchange."""
     with Ranks(KINDS[kind], 1001, 2, precision=precision) as x:
         x.attach()
@@ -73,8 +70,8 @@ def test_wait_kernel_grid_stride_and_tail(capi, exchange_env, world, n):
 
 def test_128_thread_step_kernel_forwards_its_rows(capi, exchange_env):
     """Pendulum with 140,001 envs per rank is above 132 * 8 * 128, so the step kernel runs
-    128-thread CTAs and its fused epilogue is peer_forward_rows<128> (bench.py's classic config
-    at 2 GPUs has 524,288 per rank)."""
+    128-thread CTAs into its ring slot and push_kernel forwards the rows (bench.py's classic
+    config at 2 GPUs has 524,288 per rank)."""
     with Ranks(KINDS["Pendulum"], 140_001, 2) as x:
         x.attach()
         x.reset()
@@ -123,9 +120,9 @@ def test_chains_at_every_ring_depth_and_slot_phase(depth):
 
 @pytest.mark.parametrize("block", [128])
 def test_step_kernel_cta_sizes(block):
-    """ENVPOOL_B200_STEP_BLOCK = 128 (read once per process): the fused epilogue of the
-    wider step kernel, for rows of 12 (Pendulum, Blackjack obs), 24 + 8 (Acrobot) and 100
-    bytes (Minesweeper's action mask), none a multiple of 16."""
+    """ENVPOOL_B200_STEP_BLOCK = 128 (read once per process): the wider step kernel writes
+    its ring slot before push_kernel forwards it, for rows of 12 (Pendulum, Blackjack obs),
+    24 + 8 (Acrobot) and 100 bytes (Minesweeper's action mask), none a multiple of 16."""
     _run_group(f"block{block}", STEP_BLOCK=block)
 
 
@@ -146,7 +143,7 @@ def kinds_group():
 def test_push_kernel_every_kind(kinds_group, kind, precision):
     """push_kernel on every kind's wire columns: captured exchanged chains of D + 1 steps put
     the pushes on branches beside the step chain, 40 steps with envs resetting through the
-    exchange (direct steps forward through the fused epilogue instead)."""
+    exchange (direct steps push behind the step on its own stream instead)."""
     out = kinds_group
     assert out.returncode == 0 and f"kinds {kind.name}-{precision}: " in out.stdout, \
         out.stdout[-3000:] + out.stderr[-3000:]

@@ -353,10 +353,10 @@ def test_forced_step_kernel_block(block):
 from exchange_cases import PgxKind, Ranks  # noqa: E402
 
 
-@pytest.mark.parametrize("game", GAMES, ids=lambda g: f"fused-{g}")
+@pytest.mark.parametrize("game", GAMES)
 def test_exchange(game):
-    """Direct exchanged steps (the step kernel's fused epilogue forwards both player rows) byte
-    for byte against the un-exchanged twins, and the twins against the oracle."""
+    """Direct exchanged steps (push_kernel forwards both player rows behind the step kernel)
+    byte for byte against the un-exchanged twins, and the twins against the oracle."""
     import torch
 
     n, W = 1001, 2
