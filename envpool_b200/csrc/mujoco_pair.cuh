@@ -85,6 +85,29 @@ HCP_FN double xch(const Ctx& c, double v) {
 // own + partner's: bit-identical on both lanes
 HCP_FN double psum(const Ctx& c, double v) { return v + xch(c, v); }
 
+// Solver branch trace of the host test build (HCP_STATS; tests/hc_pair_host/pair_stats.cc
+// provides hcp_trace).  Each lane reports every branch its solver takes, as (event, value):
+#if defined(HCP_STATS)
+enum {
+  TR_ROWS = 1,  // start of a constraint solve; value: rows of both lanes (0 = free flight)
+  TR_WARM,      // warm start; value: 1 if qacc_smooth was taken, + 2 if cw == cs
+  TR_LS,        // a Newton step's line search; value: TR_RUN, TR_SKIP_GS (!(gs < 0)), TR_SKIP_TOL
+  TR_UPD,       // a line-search update of alpha; value: TR_NEWTON, TR_EXPAND, TR_BISECT
+  TR_LS_END,    // how a line search that ran ended; value: TR_CONV, TR_STALL, TR_CAP
+  TR_EXIT,      // how the Newton loop ended; value: TR_GRAD0, TR_COST, TR_GRAD, TR_MAXITER, TR_ALPHA0
+};
+enum { TR_RUN = 0, TR_SKIP_GS, TR_SKIP_TOL };
+enum { TR_NEWTON = 0, TR_EXPAND, TR_BISECT };
+enum { TR_CONV = 0, TR_STALL, TR_CAP };
+enum { TR_GRAD0 = 0, TR_COST, TR_GRAD, TR_MAXITER, TR_ALPHA0 };
+#define HCP_TRACE(c, ev, val) hcp_trace((c).side, (ev), (val))
+// ... and the qacc_smooth it computed (root part, own leg part)
+#define HCP_TRACE_SMOOTH(c, r, l) hcp_trace_smooth((c).side, (r), (l))
+#else
+#define HCP_TRACE_SMOOTH(c, r, l) ((void)0)
+#define HCP_TRACE(c, ev, val) ((void)0)
+#endif
+
 // Row r of this lane: in shared memory (r < ks; field f at p[f * stride], stride = threads per
 // CTA, a compile-time constant on the device so every access is an LDS with an immediate
 // offset) or in the thread-local overflow (contiguous).  `with_row` runs `body` on whichever it
@@ -350,6 +373,7 @@ HCP_FN void pair_substep(const Ctx& c, const HcModel& cm, const LegModel& L, Pai
 #pragma unroll
   for (int i = 0; i < 3; ++i) { asr[i] = fsr[i]; asl[i] = fsl[i]; }
   pair_apply(c, FM, asr, asl);
+  HCP_TRACE_SMOOTH(c, asr, asl);
   // ---- collision + constraint rows of this lane ------------------------------------------------
   int n = 0;
 #pragma unroll
@@ -429,6 +453,7 @@ HCP_FN void pair_substep(const Ctx& c, const HcModel& cm, const LegModel& L, Pai
   // ---- constraint solve (Newton, exact line search), pair-cooperative ------------------------
   double ar[3], al[3], fcr[3], fcl[3];
   const double ntot = psum(c, (double)n);
+  HCP_TRACE(c, TR_ROWS, (int)ntot);
   if (ntot == 0) {
 #pragma unroll
     for (int i = 0; i < 3; ++i) { ar[i] = asr[i]; al[i] = asl[i]; fcr[i] = 0; fcl[i] = 0; }
@@ -452,6 +477,7 @@ HCP_FN void pair_substep(const Ctx& c, const HcModel& cm, const LegModel& L, Pai
       cw = gw + psum(c, cw);
       cs = psum(c, cs);
       const bool use_smooth = cw > cs;
+      HCP_TRACE(c, TR_WARM, (use_smooth ? 1 : 0) + (cw == cs ? 2 : 0));
 #pragma unroll
       for (int i = 0; i < 3; ++i) {
         ar[i] = use_smooth ? asr[i] : s.wr[i];
@@ -460,9 +486,6 @@ HCP_FN void pair_substep(const Ctx& c, const HcModel& cm, const LegModel& L, Pai
     }
     const double scale = 1.0 / (cm.meaninertia * hcm::NV);
     double cost = 0;
-#if defined(HCP_STATS)
-    int st_newton = 0;
-#endif
     for (int iter = 0; iter <= cm.max_iter; ++iter) {
       pair_mv(c, M, ar, al, Mar, Mal);
       Arrow H = M;
@@ -512,12 +535,19 @@ HCP_FN void pair_substep(const Ctx& c, const HcModel& cm, const LegModel& L, Pai
       g2 += psum(c, g2o);
       const double gnorm = sqrt(g2);
       if (iter > 0) {
-        if (scale * (cost - newcost) < cm.tolerance || scale * gnorm < cm.tolerance) break;
+        if (scale * (cost - newcost) < cm.tolerance || scale * gnorm < cm.tolerance) {
+          HCP_TRACE(c, TR_EXIT, scale * (cost - newcost) < cm.tolerance ? TR_COST : TR_GRAD);
+          break;
+        }
       } else if (scale * gnorm < cm.tolerance) {
+        HCP_TRACE(c, TR_EXIT, TR_GRAD0);
         break;
       }
       cost = newcost;
-      if (iter == cm.max_iter) break;
+      if (iter == cm.max_iter) {
+        HCP_TRACE(c, TR_EXIT, TR_MAXITER);
+        break;
+      }
       Fac FH;
       pair_factor(c, H, FH);
 #pragma unroll
@@ -553,10 +583,11 @@ HCP_FN void pair_substep(const Ctx& c, const HcModel& cm, const LegModel& L, Pai
       // prints the statistics of the host build).
       const double gtol = cm.tolerance * 0.01 * sqrt(sn2) / scale;
       double alpha = 0;
-#if defined(HCP_STATS)
-      int st_ls = 0;
-#endif
+      HCP_TRACE(c, TR_LS, !(gs < 0) ? TR_SKIP_GS : (fabs(gs) < gtol ? TR_SKIP_TOL : TR_RUN));
       if (gs < 0 && !(fabs(gs) < gtol)) {
+#if defined(HCP_STATS)
+        int ls_end = TR_CAP;
+#endif
         double lo = 0, hi = INFINITY;
         alpha = 1.0;
         double d1o = 0, d2o = 0;
@@ -570,9 +601,6 @@ HCP_FN void pair_substep(const Ctx& c, const HcModel& cm, const LegModel& L, Pai
           }
         });
         for (int k = 1; k < cm.ls_iter; ++k) {
-#if defined(HCP_STATS)
-          ++st_ls;
-#endif
           if (k > 1) {
             d1o = 0;
             d2o = 0;
@@ -587,29 +615,37 @@ HCP_FN void pair_substep(const Ctx& c, const HcModel& cm, const LegModel& L, Pai
           }
           const double d1 = (q1 + alpha * q2) + psum(c, d1o);
           const double d2 = q2 + psum(c, d2o);
-          if (fabs(d1) < gtol) break;
+          if (fabs(d1) < gtol) {
+#if defined(HCP_STATS)
+            ls_end = TR_CONV;
+#endif
+            break;
+          }
           if (d1 < 0) lo = alpha; else hi = alpha;
           double next = alpha - d1 / d2;
+#if defined(HCP_STATS)
+          const int upd = (next > lo && next < hi) ? TR_NEWTON : (hi == INFINITY ? TR_EXPAND : TR_BISECT);
+#endif
           if (!(next > lo && next < hi)) next = (hi == INFINITY) ? 2 * alpha + 1 : 0.5 * (lo + hi);
-          if (next == alpha) break;
+          if (next == alpha) {
+#if defined(HCP_STATS)
+            ls_end = TR_STALL;
+#endif
+            break;
+          }
+          HCP_TRACE(c, TR_UPD, upd);
           alpha = next;
         }
+        HCP_TRACE(c, TR_LS_END, ls_end);
       }
-#if defined(HCP_STATS)
-      ++st_newton;
-      if (c.side == 0) ++g_ls_hist[st_ls < 63 ? st_ls : 63];
-#endif
-      if (alpha == 0) break;
+      if (alpha == 0) {
+        HCP_TRACE(c, TR_EXIT, TR_ALPHA0);
+        break;
+      }
 #pragma unroll
       for (int i = 0; i < 3; ++i) { ar[i] += alpha * sr[i]; al[i] += alpha * sl[i]; }
     }
-#if defined(HCP_STATS)
-    if (c.side == 0) ++g_newton_hist[st_newton < 31 ? st_newton : 31];
-#endif
   }
-#if defined(HCP_STATS)
-  if (c.side == 0) ++g_rows_hist[(int)ntot < 31 ? (int)ntot : 31];
-#endif
   // ---- mj_Euler with implicit joint damping -------------------------------------------------------
   {
     Arrow E = M;

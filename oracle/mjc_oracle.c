@@ -267,6 +267,7 @@ const double* mjc_qvel(const mjc_data* d) { return d->qvel; }
 double* mjc_qpos_mut(mjc_data* d) { return d->qpos; }
 double* mjc_qvel_mut(mjc_data* d) { return d->qvel; }
 double* mjc_warm_mut(mjc_data* d) { return d->qacc_warmstart; }
+double* mjc_ctrl_mut(mjc_data* d) { return d->ctrl; }
 int mjc_nefc(const mjc_data* d) { return d->nefc; }
 
 int mjc_model_constants(const mjc_model* m, double* out, int cap) {
@@ -460,6 +461,32 @@ static void make_constraints(const mjc_model* m, const double* q, const double* 
 /* ------------------------------------------------------------------------- solver --- */
 static long g_ls_hist[64]; /* diagnostics: histogram of line-search evaluations per Newton step */
 void mjc_debug_ls_hist(long* out) { for (int i = 0; i < 64; ++i) { out[i] = g_ls_hist[i]; g_ls_hist[i] = 0; } }
+
+/* Solver branch trace: (event, value) pairs with the event and value codes of the pair kernel's
+ * host test build (envpool_b200/csrc/mujoco_pair.cuh, HCP_STATS), plus TR_CONTACTS.  Recorded
+ * only while mjc_solver_trace has been given a buffer. */
+enum { TR_ROWS = 1, TR_WARM, TR_LS, TR_UPD, TR_LS_END, TR_EXIT, TR_CONTACTS };
+enum { TR_RUN = 0 };
+enum { TR_NEWTON = 0, TR_EXPAND, TR_BISECT };
+enum { TR_CONV = 0, TR_STALL, TR_CAP };
+enum { TR_GRAD0 = 0, TR_COST, TR_GRAD, TR_MAXITER, TR_ALPHA0 };
+static int* g_trace;
+static int g_trace_cap, g_trace_len;
+static void trace(int ev, int val) {
+  if (!g_trace) return;
+  if (g_trace_len + 2 <= g_trace_cap) {
+    g_trace[g_trace_len] = ev;
+    g_trace[g_trace_len + 1] = val;
+  }
+  g_trace_len += 2;
+}
+int mjc_solver_trace(int* out, int cap) {
+  const int n = g_trace_len;
+  g_trace = out;
+  g_trace_cap = out ? cap : 0;
+  g_trace_len = 0;
+  return n;
+}
 /* cost(a) = 1/2 (a - a_s)^T M (a - a_s) + sum_i 1/2 D_i min(0, J_i a - aref_i)^2 */
 static double constraint_cost(const efc_t* e, const double* jar) {
   double c = 0;
@@ -499,6 +526,7 @@ static void solve_newton(const mjc_model* m, const efc_t* e, const double* M,
     }
     cs = constraint_cost(e, jar);
     memcpy(qacc, cw > cs ? qacc_smooth : warm, sizeof(double) * NV);
+    trace(TR_WARM, (cw > cs ? 1 : 0) + (cw == cs ? 2 : 0));
   }
   const double scale = 1.0 / (m->meaninertia * NV);
   double cost = 0;
@@ -533,14 +561,19 @@ static void solve_newton(const mjc_model* m, const efc_t* e, const double* M,
     if (iter > 0) {
       double improvement = scale * (cost - newcost);
       if (improvement < m->tolerance || scale * gnorm < m->tolerance) {
+        trace(TR_EXIT, improvement < m->tolerance ? TR_COST : TR_GRAD);
         cost = newcost;
         break;
       }
     } else if (scale * gnorm < m->tolerance) {
+      trace(TR_EXIT, TR_GRAD0);
       break;
     }
     cost = newcost;
-    if (iter == m->max_iter) break;
+    if (iter == m->max_iter) {
+      trace(TR_EXIT, TR_MAXITER);
+      break;
+    }
     ++*niter;
     /* Newton direction */
     chol9(H, L);
@@ -565,7 +598,8 @@ static void solve_newton(const mjc_model* m, const efc_t* e, const double* M,
     for (int i = 0; i < NV; ++i) snorm += search[i] * search[i];
     const double gtol = m->tolerance * 0.01 * sqrt(snorm) / scale;
     double lo = 0, hi = INFINITY, alpha = 0;
-    int ls_evals = 0;
+    int ls_evals = 0, ls_end = TR_CAP;
+    trace(TR_LS, TR_RUN);
     for (int k = 0; k < m->ls_iter; ++k) {
       ++ls_evals;
       double d1 = q1 + alpha * q2, d2 = q2;
@@ -576,15 +610,27 @@ static void solve_newton(const mjc_model* m, const efc_t* e, const double* M,
           d2 += e->D[r] * Jv[r] * Jv[r];
         }
       }
-      if (fabs(d1) < gtol) break;
+      if (fabs(d1) < gtol) {
+        ls_end = TR_CONV;
+        break;
+      }
       if (d1 < 0) lo = alpha; else hi = alpha;
       double next = alpha - d1 / d2;
+      const int upd = (next > lo && next < hi) ? TR_NEWTON : (isinf(hi) ? TR_EXPAND : TR_BISECT);
       if (!(next > lo && next < hi)) next = isinf(hi) ? 2 * alpha + 1 : 0.5 * (lo + hi);
-      if (next == alpha) break;
+      if (next == alpha) {
+        ls_end = TR_STALL;
+        break;
+      }
+      trace(TR_UPD, upd);
       alpha = next;
     }
+    trace(TR_LS_END, ls_end);
     g_ls_hist[ls_evals < 63 ? ls_evals : 63]++;
-    if (alpha == 0) break;
+    if (alpha == 0) {
+      trace(TR_EXIT, TR_ALPHA0);
+      break;
+    }
     for (int i = 0; i < NV; ++i) qacc[i] += alpha * search[i];
   }
 }
@@ -612,6 +658,8 @@ static void forward(const mjc_model* m, mjc_data* d, double* M, double* qfrc_smo
   chol9(M, L);
   chol_solve9(L, qfrc_smooth, qacc_smooth);
   d->nefc = e.n;
+  trace(TR_ROWS, e.n);
+  trace(TR_CONTACTS, d->ncon);
   solve_newton(m, &e, M, qfrc_smooth, qacc_smooth, d->qacc_warmstart, d->qacc,
                qfrc_constraint, &d->niter);
 }

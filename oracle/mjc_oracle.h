@@ -29,6 +29,7 @@ const double* mjc_qvel(const mjc_data* d);
 double* mjc_qpos_mut(mjc_data* d);
 double* mjc_qvel_mut(mjc_data* d);
 double* mjc_warm_mut(mjc_data* d); /* qacc_warmstart */
+double* mjc_ctrl_mut(mjc_data* d); /* ctrl (mjc_step overwrites it with its action) */
 /* mj_forward on the current qpos/qvel (used by tests to set a state) */
 void mjc_forward(const mjc_model* m, mjc_data* d);
 /* number of active constraint rows after the last forward/step (diagnostics) */
@@ -43,6 +44,10 @@ int mjc_debug_solve(const mjc_model* m, mjc_data* d, double* M_out, double* qfrc
                     double* qacc_out);
 double mjc_debug_dynamics(const mjc_model* m, const double* qpos, const double* qvel,
                           double* M_out, double* bias_out);
+/* Solver branch trace: from now on, (event, value) pairs of every branch the constraint solver
+ * takes go to out[0 .. cap) (out = NULL: nowhere).  Returns the number of ints the previous
+ * recording produced, which may exceed its cap.  Codes: mjc_oracle.c. */
+int mjc_solver_trace(int* out, int cap);
 
 #ifdef __cplusplus
 }

@@ -27,6 +27,7 @@ def main():
     H = ctypes.CDLL(so)
     vp = ctypes.c_void_p
     H.hc_pair_host_step.argtypes = [ctypes.c_char_p, vp, vp, vp, vp, ctypes.c_int, ctypes.c_int]
+    H.hc_pair_trace.argtypes = [ctypes.c_int, vp, ctypes.c_int]
     blob = _capi.hc_model_blob()
     rng = np.random.default_rng(0)
     for _ in range(envs):   # the env's reset distribution, uniform random actions, frame_skip 5
@@ -35,9 +36,26 @@ def main():
             a = rng.uniform(-1, 1, 6)
             H.hc_pair_host_step(blob, q.ctypes.data, v.ctypes.data, w.ctypes.data, a.ctypes.data,
                                 5, 27)
-    nh, lh, rh = (ctypes.c_long * 32)(), (ctypes.c_long * 64)(), (ctypes.c_long * 32)()
-    H.stats(nh, lh, rh)
-    nh, lh, rh = np.array(nh[:]), np.array(lh[:]), np.array(rh[:])
+    nh, lh, rh = np.zeros(32, np.int64), np.zeros(64, np.int64), np.zeros(32, np.int64)
+    cap = H.hc_pair_trace(0, None, 0)
+    tr = np.zeros(cap, np.int32)
+    H.hc_pair_trace(0, tr.ctypes.data, cap)
+    newton = passes = 0
+    for ev, val in tr.reshape(-1, 2):                 # event codes: mujoco_pair.cuh, TR_*
+        if ev == 1:                                   # a constraint solve starts
+            rh[min(val, 31)] += 1
+        elif ev == 3:                                 # a Newton step's line search
+            newton += 1
+            passes = 0
+            if val != 0:                              # skipped: no row pass
+                lh[0] += 1
+        elif ev == 4:                                 # an update of alpha, after a row pass
+            passes += 1
+        elif ev == 5:                                 # ended; converged or stalled on a pass
+            lh[min(passes + (val != 2), 63)] += 1
+        elif ev == 6:                                 # the Newton loop ends
+            nh[min(newton, 31)] += 1
+            newton = 0
     print("merged constraint rows per mj_step:", {i: int(x) for i, x in enumerate(rh) if x},
           f"-> {100 * rh[0] / rh.sum():.0f} % of the mj_steps have none")
     print("line searches per constrained mj_step:", {i: int(x) for i, x in enumerate(nh) if x},
