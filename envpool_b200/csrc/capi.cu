@@ -1083,6 +1083,40 @@ int exchange_step(epb_pool* p, const void* d_action, cudaStream_t s, int chain_k
                   cudaEvent_t step_done = nullptr);
 int exchange_wait_launch(epb_pool* p, cudaStream_t s);
 
+// The node that the next node captured on `st` would depend on alone: the step just captured.
+int captured_tail(cudaStream_t st, cudaGraphNode_t* node) {
+  cudaStreamCaptureStatus cs;
+  const cudaGraphNode_t* deps = nullptr;
+  const cudaGraphEdgeData* data = nullptr;
+  size_t n = 0;
+  EPB_CUDA(cudaStreamGetCaptureInfo_v3(st, &cs, nullptr, nullptr, &deps, &data, &n));
+  *node = n == 1 ? deps[0] : nullptr;
+  return EPB_OK;
+}
+
+// Before the next step node captured on `st`: its edge from `prev` (the step before it) becomes
+// programmatic -- its grid launches while `prev` drains, and griddepcontrol.wait holds every
+// access back until `prev` has completed and its stores are visible.  Its other edges (the
+// join of a refill branch, of the exchange wait and push branches) are set to full
+// dependencies: a launch with the PDL attribute would make those programmatic as well.
+int program_step_edge(cudaStream_t st, cudaGraphNode_t prev) {
+  cudaStreamCaptureStatus cs;
+  const cudaGraphNode_t* deps = nullptr;
+  const cudaGraphEdgeData* data = nullptr;
+  size_t n = 0;
+  EPB_CUDA(cudaStreamGetCaptureInfo_v3(st, &cs, nullptr, nullptr, &deps, &data, &n));
+  std::vector<cudaGraphNode_t> nodes(deps, deps + n);
+  std::vector<cudaGraphEdgeData> edges(n);  // zero: a full dependency
+  for (size_t i = 0; i < n; ++i) {
+    if (nodes[i] != prev) continue;
+    edges[i].from_port = cudaGraphKernelNodePortProgrammatic;
+    edges[i].type = cudaGraphDependencyTypeProgrammatic;
+  }
+  EPB_CUDA(cudaStreamUpdateCaptureDependencies_v2(st, nodes.data(), edges.data(), n,
+                                                  cudaStreamSetCaptureDependencies));
+  return EPB_OK;
+}
+
 // K consecutive sync steps on `st`, step k reading action row (t0 + k) % T.  `fork` (only
 // while capturing) puts the off-critical-path kernels on parallel graph branches:
 //   * record envs: one refill on p->side after every refill_every-th step (and after the
@@ -1095,7 +1129,13 @@ int exchange_wait_launch(epb_pool* p, cudaStream_t s);
 //     the batch of step k is still arriving; step k+D-1 waits for it (its credit needs the
 //     local release as well as the peers');
 //   * timing marks: ev0 takes the timestamp at which step mark0 became ready, ev1 the
-//     completion of step mark1-1 -- recorded on a branch of their own, not in series.
+//     completion of step mark1-1 -- recorded on a branch of their own, not in series.  Both
+//     hang off a step node by a full edge; step mark0 may launch earlier, but it waits for
+//     step mark0-1 to complete, the moment ev0 takes.
+// `fork` also makes each step's edge from the step before it programmatic (program_step_edge)
+// for the kinds whose step kernel allows it (KindLaunch::programmatic_step): nothing but
+// kernel nodes ever sits between two steps on `st`, and every join stays a full dependency, so
+// the refill bound above holds as it is.  HalfCheetah's pair kernel keeps plain edges.
 int run_chain(epb_pool* p, cudaStream_t st, const ChainKey& c, bool fork, cudaEvent_t ev0,
               cudaEvent_t ev1) {
   const size_t row = (size_t)p->act.row_bytes * p->N;
@@ -1106,6 +1146,11 @@ int run_chain(epb_pool* p, cudaStream_t st, const ChainKey& c, bool fork, cudaEv
   int nref = 0;          // refills launched so far in this chain
   bool after_trigger = false;
   const int D = p->x_depth;
+  const bool pdl = fork && p->fn.programmatic_step;
+  cudaGraphNode_t prev = nullptr;  // pdl: the step node captured last
+  auto program_edge = [&]() -> int {
+    return pdl && prev ? program_step_edge(st, prev) : EPB_OK;
+  };
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   cudaStreamIsCapturing(st, &cap);
   const bool capturing = cap != cudaStreamCaptureStatusNone;
@@ -1151,6 +1196,8 @@ int run_chain(epb_pool* p, cudaStream_t st, const ChainKey& c, bool fork, cudaEv
         // Round trips cannot be shortened, so they are overlapped.
         if (k >= D) EPB_CUDA(cudaStreamWaitEvent(st, p->x_ev_push[(k - D) % D], 0));
         cudaStream_t ps = p->x_push[k % 3];
+        rc = program_edge();
+        if (rc != EPB_OK) return rc;
         rc = exchange_step(p, a, st, rec ? -2 : -1, nx, ps, p->x_ev_step[k % D]);
         if (rc != EPB_OK) return rc;
         EPB_CUDA(cudaEventRecord(p->x_ev_push[k % D], ps));
@@ -1165,7 +1212,13 @@ int run_chain(epb_pool* p, cudaStream_t st, const ChainKey& c, bool fork, cudaEv
         if (rc != EPB_OK) return rc;
       }
     } else {
+      rc = program_edge();
+      if (rc != EPB_OK) return rc;
       rc = launch_batch(p, a, nullptr, p->N, 0, p->d_slab, st, rec ? -2 : -1, nullptr, nx);
+      if (rc != EPB_OK) return rc;
+    }
+    if (pdl) {
+      rc = captured_tail(st, &prev);
       if (rc != EPB_OK) return rc;
     }
     if (rec && ((k % R) == R - 1 || k == c.K - 1)) {

@@ -505,7 +505,8 @@ step_kernel(StateView sv, OutView ov, const typename Env::Act* __restrict__ acti
   // here for the previous kernel of the stream.  Every global load sits BEHIND the wait:
   // the action / env_ids of the device-resident path are usually written by the kernel just
   // before this one (a policy's argmax), and state and slab belong to the previous step.
-  // Both instructions are no-ops when the kernel is launched without the PDL attribute.
+  // Both instructions are no-ops when nothing upstream is programmatic: the kernel is launched
+  // without the PDL attribute and no programmatic graph edge leads into it.
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");
   if (active) {
@@ -717,9 +718,11 @@ cudaError_t launch_step_b(const LaunchArgs& a) {
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  // PDL pays off for direct launches (hides part of the launch latency of every step); inside
-  // a captured graph the programmatic edges measured slower than plain kernel->kernel edges, so
-  // captures keep full serialisation.
+  // Direct launches carry the PDL attribute: the next step's grid launches while this one
+  // drains.  Captured launches do not: stream capture would make every edge into the node
+  // programmatic, joins from other branches included.  Engine-captured chains set the edge
+  // from the previous step themselves (capi.cu, run_chain); a capture driven by the caller
+  // keeps plain edges, since the node before may be one of the caller's.
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   cudaStreamIsCapturing(a.stream, &cap);
   cfg.numAttrs = cap == cudaStreamCaptureStatusNone ? 1 : 0;
@@ -768,6 +771,9 @@ struct KindLaunch {
   // added to bytes_per_env_step's count of action, state and columns: per-step RNG traffic,
   // less any state words a step does not touch
   int extra_step_bytes;
+  // `step` launches step_kernel, whose global accesses all sit behind griddepcontrol.wait:
+  // engine-captured chains may give it a programmatic edge from the step before (run_chain)
+  bool programmatic_step = false;
 };
 
 struct KindDesc {
@@ -799,7 +805,7 @@ template <class Env>
 KindLaunch kind_launch(int extra_step_bytes = 0) {
   launch_fn refill = nullptr;
   if constexpr (UsesRec<Env>::value) refill = launch_refill<Env>;
-  return {launch_step<Env>, launch_rollout<Env>, refill, extra_step_bytes};
+  return {launch_step<Env>, launch_rollout<Env>, refill, extra_step_bytes, true};
 }
 // the launch of a kind whose kernels depend on neither precision nor iopt
 template <class Env, int kExtraStepBytes = 0>
