@@ -30,6 +30,11 @@ KINDS = {
 # ... and of the kinds with two players per env, whose per-player columns hold two rows per env
 # row (epb_state_key_players).  Kept apart: code that walks KINDS sees one-player pools only.
 TWO_PLAYER_KINDS = {"TicTacToe": 14, "ConnectFour": 15}
+# ... and the two-player kinds added after those, with fixtures of their own
+# (tests/golden/pgx/hex_othello/).
+TWO_PLAYER_KINDS_2 = {"Hex": 16, "Othello": 17}
+# every kind by task name: what CPool resolves a task through
+ALL_KINDS = {**KINDS, **TWO_PLAYER_KINDS, **TWO_PLAYER_KINDS_2}
 DTYPES = {0: np.int32, 1: np.float32, 2: np.float64, 3: np.bool_}
 
 # every symbol include/envpool_b200.h declares (checked by tests/test_abi.py)
@@ -220,7 +225,7 @@ class CPool:
         cfg.forward_reward_weight = forward_reward_weight
         cfg.reset_noise_scale = reset_noise_scale
         h = ctypes.c_void_p()
-        kind = KINDS[task] if task in KINDS else TWO_PLAYER_KINDS[task]
+        kind = ALL_KINDS[task]
         _check(L.epb_create(kind, ctypes.byref(cfg), ctypes.byref(h)))
         self.h = h
         self.task = task

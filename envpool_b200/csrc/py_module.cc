@@ -111,6 +111,7 @@ struct EnvDesc {
   int kind;
   std::vector<std::string> cfg_keys;   // env-specific keys (XxxEnvFns::DefaultConfig)
   py::tuple (*cfg_defaults)();
+  int players = 1;  // players per env: the max_num_players a pool of this kind must be given
 };
 
 constexpr int kNumCommon = 10;
@@ -362,10 +363,14 @@ class SpecBase {
         action_cols.push_back(colb("action", 'i', {-1, 2}, 0, 9));
         break;
       case EPB_TIC_TAC_TOE:  // pgx/board_games.h TicTacToeEnvFns
-      case EPB_CONNECT_FOUR: {  // pgx/board_games.h ConnectFourEnvFns
-        const bool ttt = desc->kind == EPB_TIC_TAC_TOE;
-        const int rows = ttt ? 3 : 6, cols = ttt ? 3 : 7, actions = ttt ? 9 : 7;
-        state_cols.push_back(col("obs", 'b', {-1, rows, cols, 2}));
+      case EPB_CONNECT_FOUR:  // pgx/board_games.h ConnectFourEnvFns
+      case EPB_HEX:           // pgx/board_games.h HexEnvFns
+      case EPB_OTHELLO: {     // pgx/board_games.h OthelloEnvFns
+        const int k = desc->kind;
+        const int rows = k == EPB_TIC_TAC_TOE ? 3 : k == EPB_CONNECT_FOUR ? 6 : k == EPB_HEX ? 11 : 8;
+        const int cols = k == EPB_TIC_TAC_TOE ? 3 : k == EPB_CONNECT_FOUR ? 7 : rows;
+        const int actions = k == EPB_TIC_TAC_TOE ? 9 : k == EPB_CONNECT_FOUR ? 7 : rows * cols + 1;
+        state_cols.push_back(col("obs", 'b', {-1, rows, cols, k == EPB_HEX ? 4 : 2}));
         state_cols.push_back(col("info:board", 'i', {rows, cols}));
         state_cols.push_back(col("info:current_player", 'i', {}));
         state_cols.push_back(col("info:legal_action_mask", 'b', {actions}));
@@ -413,16 +418,16 @@ class PoolBase {
 
   void Create(const SpecBase& spec, int device, const std::string& precision,
               int env_id_offset) {
-    const bool two_players =
-        spec.desc->kind == EPB_TIC_TAC_TOE || spec.desc->kind == EPB_CONNECT_FOUR;
-    if (two_players) {
-      if (spec.cfg<int>("max_num_players") != 2)
-        throw std::invalid_argument(std::string(spec.desc->name) +
-                                    " is a two-player game: max_num_players must be 2");
+    players = spec.desc->players;
+    if (players > 1) {
+      if (spec.cfg<int>("max_num_players") != players)
+        throw std::invalid_argument(std::string(spec.desc->name) + " is a " +
+                                    (players == 2 ? "two" : std::to_string(players)) +
+                                    "-player game: max_num_players must be " +
+                                    std::to_string(players));
     } else if (spec.cfg<int>("max_num_players") != 1) {
       throw std::invalid_argument("max_num_players != 1 is outside the accelerated path");
     }
-    players = two_players ? 2 : 1;
     if (spec.desc->kind == EPB_HALF_CHEETAH) {
       // post_constraint (v5) only adds mj_rnePostConstraint (mujoco_env.h:145-147), whose
       // outputs (cacc/cfrc_*) HalfCheetah never reads: accepted, no effect on any column.
@@ -684,6 +689,9 @@ void register_env(py::module_& m, const EnvDesc* d) {
 
 #define DESC(NAME, KIND, KEYS, DEFAULTS)                                   \
   static EnvDesc desc_##NAME{#NAME, KIND, KEYS, []() -> py::tuple DEFAULTS}
+// a kind with more than one player per env
+#define DESC_PLAYERS(NAME, KIND, PLAYERS, KEYS, DEFAULTS)                  \
+  static EnvDesc desc_##NAME{#NAME, KIND, KEYS, []() -> py::tuple DEFAULTS, PLAYERS}
 
 using S = std::vector<std::string>;
 
@@ -751,12 +759,19 @@ PYBIND11_MODULE(EPB_MODULE_NAME, m) {
        });
   register_env<EPB_HALF_CHEETAH>(m, &desc_GymHalfCheetah);
 #elif defined(EPB_FAMILY_PGX)
-  // pgx/pgx.cc (TicTacToe and ConnectFour: the two-player board games on the hot path)
-  DESC(TicTacToe, EPB_TIC_TAC_TOE, S{"task"}, { return py::make_tuple(std::string("tic_tac_toe")); });
-  DESC(ConnectFour, EPB_CONNECT_FOUR, S{"task"},
-       { return py::make_tuple(std::string("connect_four")); });
+  // pgx/pgx.cc (TicTacToe, ConnectFour, Hex and Othello: the two-player board games on the
+  // hot path)
+  DESC_PLAYERS(TicTacToe, EPB_TIC_TAC_TOE, 2, S{"task"},
+               { return py::make_tuple(std::string("tic_tac_toe")); });
+  DESC_PLAYERS(ConnectFour, EPB_CONNECT_FOUR, 2, S{"task"},
+               { return py::make_tuple(std::string("connect_four")); });
+  DESC_PLAYERS(Hex, EPB_HEX, 2, S{"task"}, { return py::make_tuple(std::string("hex")); });
+  DESC_PLAYERS(Othello, EPB_OTHELLO, 2, S{"task"},
+               { return py::make_tuple(std::string("othello")); });
   register_env<EPB_TIC_TAC_TOE>(m, &desc_TicTacToe);
   register_env<EPB_CONNECT_FOUR>(m, &desc_ConnectFour);
+  register_env<EPB_HEX>(m, &desc_Hex);
+  register_env<EPB_OTHELLO>(m, &desc_Othello);
 #else
 #error "define one EPB_FAMILY_* macro"
 #endif

@@ -1,5 +1,5 @@
 """PGX env registration (task ids, `task` and max_num_players as in envpool/pgx/registration.py;
-TicTacToe and ConnectFour are the accelerated PGX games)."""
+TicTacToe, ConnectFour, Hex and Othello are the accelerated PGX games)."""
 from ..registration import register
 
 register(task_id="TicTacToe-v1", import_path="envpool_b200.pgx", spec_cls="TicTacToeEnvSpec",
@@ -8,3 +8,9 @@ register(task_id="TicTacToe-v1", import_path="envpool_b200.pgx", spec_cls="TicTa
 register(task_id="ConnectFour-v1", import_path="envpool_b200.pgx",
          spec_cls="ConnectFourEnvSpec", dm_cls="ConnectFourDMEnvPool",
          gymnasium_cls="ConnectFourGymnasiumEnvPool", task="connect_four", max_num_players=2)
+register(task_id="Hex-v1", import_path="envpool_b200.pgx", spec_cls="HexEnvSpec",
+         dm_cls="HexDMEnvPool", gymnasium_cls="HexGymnasiumEnvPool", task="hex",
+         max_num_players=2)
+register(task_id="Othello-v1", import_path="envpool_b200.pgx", spec_cls="OthelloEnvSpec",
+         dm_cls="OthelloDMEnvPool", gymnasium_cls="OthelloGymnasiumEnvPool", task="othello",
+         max_num_players=2)

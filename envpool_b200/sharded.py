@@ -34,8 +34,9 @@ _TASK_KWARGS = {
     "Blackjack": ("natural", "sab"),
     "HalfCheetah": ("frame_skip", "ctrl_cost_weight", "forward_reward_weight",
                     "reset_noise_scale", "post_constraint", "gymnasium_v5_render_camera"),
-    "TicTacToe": ("task", "max_num_players"), "ConnectFour": ("task", "max_num_players"),
 }
+# ... and of every multi-player kind: its registration's `task` and max_num_players
+_PLAYER_KWARGS = ("task", "max_num_players")
 
 
 def shard_range(num_envs: int, rank: int, world: int) -> Tuple[int, int]:
@@ -118,12 +119,13 @@ class ShardedPool:
         _ensure_registered()
         _, spec_cls, kwargs = registry.specs[task_id]
         engine_task = spec_cls.replace("EnvSpec", "").replace("Gym", "")
+        players = kwargs.get("max_num_players", 1)  # as registered: the kind's players per env
         dropped = sorted(set(task_kwargs) - set(_COMMON_KWARGS) -
-                         set(_TASK_KWARGS.get(engine_task, ())))
+                         set(_TASK_KWARGS.get(engine_task, ())) -
+                         set(_PLAYER_KWARGS if players > 1 else ()))
         if dropped:
             raise ValueError(f"ShardedPool({task_id!r}) cannot carry {dropped} to its shards")
         kwargs = {**kwargs, **task_kwargs}
-        players = 2 if engine_task in ("TicTacToe", "ConnectFour") else 1
         if kwargs.get("max_num_players", 1) != players:
             raise ValueError(f"ShardedPool({task_id!r}): max_num_players must be {players}")
         hc = {}

@@ -1,7 +1,7 @@
-"""TicTacToe-v1 and ConnectFour-v1 env-step rates on one GPU, next to the reference's CPU thread
-pool.
+"""PGX env-step rates on one GPU, next to the reference's CPU thread pool.
 
-    python profiles/pgx_rate.py [--out FILE.json]
+    python profiles/pgx_rate.py [--games TicTacToe,ConnectFour] [--out FILE.json]
+    python profiles/pgx_rate.py --games Hex,Othello --out profiles/pgx_hex_othello_rate.json
 
 For 65536, 1M and 4M envs of each game, env-steps/s of
   * the captured per-step chain (epb_step_many_timed: CUDA-graph replay of one step launch per
@@ -13,7 +13,7 @@ with the HBM fraction epb_bytes_per_env_step x rate / 3.35 TB/s (H100 SXM HBM3 d
 A second line drives a legal-random policy on the device: between step_device calls, torch
 takes the masked argmax of uniform noise over the last step's info:legal_action_mask, the
 pattern of a self-play loop; CUDA events around 64 steps (policy kernels included).  The
-reference's own AsyncEnvPool<TicTacToeEnv> / <ConnectFourEnv> (oracle/_ref) runs on every host
+reference's own AsyncEnvPool of each game (oracle/_ref) runs on every host
 thread at 65536 envs when the build compiled it.  The card's name and power limit are read in
 the same run.  Needs a CUDA device: there is no CPU fallback.
 """
@@ -30,7 +30,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 HBM_BYTES_PER_S = 3.35e12
-ACTIONS = {"TicTacToe": 9, "ConnectFour": 7}
+ACTIONS = {"TicTacToe": 9, "ConnectFour": 7, "Hex": 122, "Othello": 65}
 
 
 def card():
@@ -43,7 +43,9 @@ def card():
 def gpu_rates(game, n, torch, CPool):
     pool = CPool(game, n, seed=1)
     rng = np.random.default_rng(0)
-    K, m0, T = 80, 16, 16
+    K, m0 = 80, 16
+    # rollout steps per launch: 16, fewer where 16 steps of outputs would not fit beside the pool
+    T = max(1, min(16, int(40e9 // (n * sum(k.row_bytes for k in pool.keys)))))
     acts = torch.from_numpy(rng.integers(0, ACTIONS[game], size=(K, n)).astype(np.int32)).cuda()
     pool.reset_device()
     chain = []
@@ -89,7 +91,7 @@ def gpu_rates(game, n, torch, CPool):
     pool.close()
     del acts, out, mask, done
     torch.cuda.empty_cache()
-    return {"num_envs": n, "bytes_per_env_step": b,
+    return {"num_envs": n, "bytes_per_env_step": b, "rollout_T": T,
             "chain_env_steps_per_s": max(chain),
             "chain_hbm_fraction": max(chain) * b / HBM_BYTES_PER_S,
             "rollout_env_steps_per_s": max(roll),
@@ -99,11 +101,13 @@ def gpu_rates(game, n, torch, CPool):
 
 
 def ref_rate(game, n):
-    from oracle import pgx_lib
+    from oracle import hex_othello_lib, pgx_lib
 
-    if not pgx_lib.ref_available():
+    lib, Ref = (hex_othello_lib, hex_othello_lib.HexOthelloRef) if game in hex_othello_lib.GAMES \
+        else (pgx_lib, pgx_lib.PgxRef)
+    if not lib.ref_available():
         return {"num_envs": n, "env_steps_per_s": "not measured (oracle/_ref was not built)"}
-    pool = pgx_lib.PgxRef(game, n, seed=1, num_threads=0)
+    pool = Ref(game, n, seed=1, num_threads=0)
     acts = np.random.default_rng(0).integers(0, ACTIONS[game], size=(16, n)).astype(np.int32)
     steps = 20
     sec = pool.bench(acts, 5, steps)
@@ -116,6 +120,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default="")
     ap.add_argument("--sizes", default="65536,1048576,4194304")
+    ap.add_argument("--games", default="TicTacToe,ConnectFour")
     args = ap.parse_args()
     import torch
 
@@ -123,11 +128,12 @@ def main():
         raise SystemExit("pgx_rate.py measures the GPU: no CUDA device")
     from envpool_b200._capi import CPool
 
-    res = {"tasks": ["TicTacToe-v1", "ConnectFour-v1"], "card": card(),
+    games = args.games.split(",")
+    res = {"tasks": [f"{g}-v1" for g in games], "card": card(),
            "hbm_bytes_per_s_datasheet": HBM_BYTES_PER_S,
            "gpu": {g: [gpu_rates(g, int(n), torch, CPool) for n in args.sizes.split(",")]
-                   for g in ACTIONS},
-           "reference_cpu": {g: ref_rate(g, 65536) for g in ACTIONS},
+                   for g in games},
+           "reference_cpu": {g: ref_rate(g, 65536) for g in games},
            "date": time.strftime("%Y-%m-%d")}
     text = json.dumps(res, indent=1)
     print(text)
