@@ -534,10 +534,11 @@ int launch_refill(epb_pool* p, cudaStream_t stream) {
 // on the same stream after every `refill_every`-th step launch -- an env consumes at most one
 // record per launch, the ring holds rec_q > refill_every.  chain_k == -2: the caller places the
 // refill itself (host path: behind the D2H copy; engine-captured chains: on a parallel graph
-// branch every refill_every steps, run_chain).
+// branch every refill_every steps, run_chain).  prev_in_slab: LaunchArgs::prev_in_slab.
 int launch_batch(epb_pool* p, const void* d_action, const int32_t* d_ids, int n,
                  int force_reset, char* d_slab, cudaStream_t stream, int chain_k = -1,
-                 int32_t* wire = nullptr, const void* next_action = nullptr) {
+                 int32_t* wire = nullptr, const void* next_action = nullptr,
+                 int prev_in_slab = 0) {
   p->d_last = d_slab;
   p->started = true;
   LaunchArgs a = launch_args(p, stream);
@@ -548,6 +549,7 @@ int launch_batch(epb_pool* p, const void* d_action, const int32_t* d_ids, int n,
   a.n = n;
   a.force_reset = force_reset;
   a.next_action = next_action;
+  a.prev_in_slab = prev_in_slab;
   EPB_CUDA(p->fn.step(a));
   ++p->launches;
   if (p->fn.refill) {
@@ -1214,7 +1216,10 @@ int run_chain(epb_pool* p, cudaStream_t st, const ChainKey& c, bool fork, cudaEv
     } else {
       rc = program_edge();
       if (rc != EPB_OK) return rc;
-      rc = launch_batch(p, a, nullptr, p->N, 0, p->d_slab, st, rec ? -2 : -1, nullptr, nx);
+      // Step k > 0 follows step k - 1 into the same slab with nothing in between (refills
+      // touch only the record rings), so it stores only the common columns that change.
+      rc = launch_batch(p, a, nullptr, p->N, 0, p->d_slab, st, rec ? -2 : -1, nullptr, nx,
+                        k > 0);
       if (rc != EPB_OK) return rc;
     }
     if (pdl) {

@@ -312,19 +312,29 @@ __global__ void seed_kernel(StateView sv, int base_seed, const int32_t* env_seed
 
 // ---------------------------------------------------------------------------------------
 // Common output columns: Env::Allocate, core/env.h:224-256.
+// prev_flags >= 0: the row already holds what the previous step of the same chain wrote from
+// its result `prev_flags` (run_chain, step_kernel's prev_in_slab), so the columns that are a
+// function of the flags alone are stored only where they change: info:env_id and
+// info:players.env_id never, done / discount / step_type / trunc around a reset or an
+// episode's end.  elapsed_step, reward and the wire word are always stored.
 __device__ __forceinline__ void write_common(const OutView& ov, int64_t row, int global_eid,
                                              int cur, int done, float reward,
-                                             int max_steps) {
+                                             int max_steps, int prev_flags = -1) {
   int step_type = (cur == 0) ? 0 : (done ? 2 : 1);
-  if (ov.env_id) ov.env_id[row] = global_eid;
-  if (ov.players_id) ov.players_id[row] = global_eid;
-  if (ov.elapsed) ov.elapsed[row] = cur;
-  if (ov.done) ov.done[row] = (uint8_t)done;
-  if (ov.reward) ov.reward[row] = reward;
-  if (ov.discount) ov.discount[row] = done ? 0.0f : 1.0f;
-  if (ov.step_type) ov.step_type[row] = step_type;
   const int trunc = done && (cur >= max_steps);
-  if (ov.trunc) ov.trunc[row] = (uint8_t)trunc;
+  const bool known = prev_flags >= 0;
+  const int pcur = prev_flags >> 1, pdone = prev_flags & 1;
+  const bool same_done = known && done == pdone;
+  const bool same_type = known && step_type == ((pcur == 0) ? 0 : (pdone ? 2 : 1));
+  const bool same_trunc = known && trunc == (pdone && (pcur >= max_steps));
+  if (ov.env_id && !known) ov.env_id[row] = global_eid;
+  if (ov.players_id && !known) ov.players_id[row] = global_eid;
+  if (ov.elapsed) ov.elapsed[row] = cur;
+  if (ov.done && !same_done) ov.done[row] = (uint8_t)done;
+  if (ov.reward) ov.reward[row] = reward;
+  if (ov.discount && !same_done) ov.discount[row] = done ? 0.0f : 1.0f;
+  if (ov.step_type && !same_type) ov.step_type[row] = step_type;
+  if (ov.trunc && !same_trunc) ov.trunc[row] = (uint8_t)trunc;
   if (ov.wire) ov.wire[row] = pack_wire(cur, done, trunc);
 }
 
@@ -365,11 +375,13 @@ template <class Env>
 struct Players<Env, typename std::enable_if<(Env::kPlayers > 1)>::type> {
   static constexpr int value = Env::kPlayers;
 };
+// prev_flags: as write_common's (-1: nothing known about the row); P = 2 stores every column.
 template <class Env>
 __device__ __forceinline__ void write_common_env(const OutView& ov, int64_t row, int global_eid,
-                                                 int flags, const StepOut& so, int max_steps) {
+                                                 int flags, const StepOut& so, int max_steps,
+                                                 int prev_flags = -1) {
   if constexpr (Players<Env>::value == 1) {
-    write_common(ov, row, global_eid, flags >> 1, flags & 1, so.reward, max_steps);
+    write_common(ov, row, global_eid, flags >> 1, flags & 1, so.reward, max_steps, prev_flags);
   } else {
     static_assert(Players<Env>::value == 2, "per-player columns: P = 1 or 2");
     write_common_pair(ov, row, global_eid, flags >> 1, flags & 1, so, max_steps);
@@ -488,11 +500,14 @@ __device__ __forceinline__ void pin_value(ActI32x2& v) {
 }
 
 // Single sync step of a batch: thread `row` handles env env_ids[row] (identity if NULL).
+// prev_in_slab: the previous kernel on the stream was this kernel over every env, identity
+// rows, into the same output rows (a step chain after its first step), so each row holds the
+// common columns of the flags this step loads (write_common's prev_flags).
 template <class Env, int kB = kBlock>
 __global__ void __launch_bounds__(kB)
 step_kernel(StateView sv, OutView ov, const typename Env::Act* __restrict__ action,
             const int32_t* __restrict__ env_ids, int n, int force_reset,
-            const typename Env::Act* __restrict__ next_action) {
+            const typename Env::Act* __restrict__ next_action, int prev_in_slab) {
   int row = blockIdx.x * kB + threadIdx.x;
   bool active = row < n;
   typename Env::State s;
@@ -530,11 +545,13 @@ step_kernel(StateView sv, OutView ov, const typename Env::Act* __restrict__ acti
     if (next_action && (threadIdx.x & 31) == 0)
       asm volatile("prefetch.global.L2 [%0];" ::"l"(next_action + row));
     pin_value(a);
+    const int prev_flags = prev_in_slab ? flags : -1;
     env_step<Env>(sv, eid, flags, s, a, force_reset != 0, so, mt_idx, rcons);
     Env::store(sv, eid, s);
     sv.flags[eid] = flags;
     if (!kRec && kRng && mt_idx != mt_idx0) sv.mt_idx[eid] = mt_idx;
-    write_common_env<Env>(ov, row, eid + sv.env_id_offset, flags, so, sv.max_steps);
+    write_common_env<Env>(ov, row, eid + sv.env_id_offset, flags, so, sv.max_steps,
+                          prev_flags);
   }
   if constexpr (Env::kBlockObs) {
     Env::template block_write_obs<kB>(ov, (int64_t)blockIdx.x * kB, n, active, s, so);
@@ -679,6 +696,9 @@ struct LaunchArgs {
   cudaStream_t stream;
   const void* next_action;  // step chains: action row of the following step (L2 prefetch)
   const void* params;       // the pool's family parameters (KindDesc::setup; HalfCheetah only)
+  // step_kernel's prev_in_slab: set by run_chain alone, for the steps after the first of a chain
+  // that writes p->d_slab (kernels that do not read it store every column anyway)
+  int prev_in_slab;
 };
 typedef cudaError_t (*launch_fn)(const LaunchArgs&);
 
@@ -728,7 +748,8 @@ cudaError_t launch_step_b(const LaunchArgs& a) {
   cfg.numAttrs = cap == cudaStreamCaptureStatusNone ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, step_kernel<Env, kB>, a.sv, a.ov,
                             static_cast<const typename Env::Act*>(a.action), a.env_ids, a.n,
-                            a.force_reset, static_cast<const typename Env::Act*>(a.next_action));
+                            a.force_reset, static_cast<const typename Env::Act*>(a.next_action),
+                            a.prev_in_slab);
 }
 
 template <class Env>
