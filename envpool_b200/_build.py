@@ -36,6 +36,7 @@ CUDA_UNITS = {
     "jumanji.cu": [],
     "mujoco.cu": [],
     "pgx.cu": [],
+    "go.cu": [],
     "capi.cu": [],
 }
 PY_MODULES = {

@@ -33,8 +33,11 @@ TWO_PLAYER_KINDS = {"TicTacToe": 14, "ConnectFour": 15}
 # ... and the two-player kinds added after those, with fixtures of their own
 # (tests/golden/pgx/hex_othello/).
 TWO_PLAYER_KINDS_2 = {"Hex": 16, "Othello": 17}
-# every kind by task name: what CPool resolves a task through
+# every kind by task name but Go's
 ALL_KINDS = {**KINDS, **TWO_PLAYER_KINDS, **TWO_PLAYER_KINDS_2}
+# ... and Go, one kind per board size (tests/golden/pgx/go/); CPool takes its komi and
+# max_terminal_steps
+GO_KINDS = {"Go9x9": 18, "Go13x13": 19, "Go19x19": 20}
 DTYPES = {0: np.int32, 1: np.float32, 2: np.float64, 3: np.bool_}
 
 # every symbol include/envpool_b200.h declares (checked by tests/test_abi.py)
@@ -50,7 +53,7 @@ ABI_SYMBOLS = [
     "epb_exchange_status", "epb_exchange_slice_bytes", "epb_exchange_depth",
     "epb_step_many_timed", "epb_step_exchange_many_device", "epb_fp64_peak_gflops",
     "epb_hc_model", "epb_hc_pair_rows", "epb_exchange_trace", "epb_game2048_boards",
-    "epb_minesweeper_config", "epb_state_key_players",
+    "epb_minesweeper_config", "epb_state_key_players", "epb_go_config",
 ]
 IPC_HANDLE_BYTES = 64
 
@@ -142,6 +145,7 @@ def load_library() -> ctypes.CDLL:
     L.epb_hc_pair_rows.argtypes = [vp, ci]
     L.epb_game2048_boards.argtypes = [vp, vp, vp]
     L.epb_minesweeper_config.argtypes = [vp, vp, vp, vp, vp]
+    L.epb_go_config.argtypes = [vp, ctypes.c_double, ctypes.c_int32]
     _lib = L
     return L
 
@@ -200,9 +204,11 @@ class CPool:
                  precision: str = "f64", env_id_offset: int = 0,
                  env_seed=None, batch_size: int = 0, frame_skip: int = 0,
                  ctrl_cost_weight: float = math.nan, forward_reward_weight: float = math.nan,
-                 reset_noise_scale: float = math.nan):
+                 reset_noise_scale: float = math.nan, komi: Optional[float] = None,
+                 max_terminal_steps: Optional[int] = None):
         """HalfCheetah: frame_skip <= 0 and NaN weights / noise scale select the reference
-        defaults (5, 0.1, 1.0, 0.1); every other value is used as given, negative included."""
+        defaults (5, 0.1, 1.0, 0.1); every other value is used as given, negative included.
+        Go: komi (default 7.5) and max_terminal_steps (default 0 = 2 S^2), epb_go_config."""
         L = load_library()
         self.lib = L
         cfg = EpbConfig()
@@ -225,7 +231,7 @@ class CPool:
         cfg.forward_reward_weight = forward_reward_weight
         cfg.reset_noise_scale = reset_noise_scale
         h = ctypes.c_void_p()
-        kind = ALL_KINDS[task]
+        kind = {**ALL_KINDS, **GO_KINDS}[task]
         _check(L.epb_create(kind, ctypes.byref(cfg), ctypes.byref(h)))
         self.h = h
         self.task = task
@@ -233,6 +239,9 @@ class CPool:
         self.device = device
         self.precision = precision
         self._owned = True
+        if komi is not None or max_terminal_steps is not None:
+            self.go_config(7.5 if komi is None else komi,
+                           0 if max_terminal_steps is None else max_terminal_steps)
         self._read_keys()
 
     @classmethod
@@ -532,6 +541,11 @@ class CPool:
             bufs.append(b)
         _check(self.lib.epb_minesweeper_config(
             self.h, *[None if b is None else b.ctypes.data for b in bufs]))
+
+    def go_config(self, komi: float, max_terminal_steps: int):
+        """Go's komi and max_terminal_steps (0 = 2 S^2); before the pool's first reset, step,
+        rollout or state import."""
+        _check(self.lib.epb_go_config(self.h, float(komi), int(max_terminal_steps)))
 
     def state_layout(self) -> Dict[str, int]:
         out = (ctypes.c_int64 * 12)()

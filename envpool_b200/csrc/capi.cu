@@ -160,6 +160,7 @@ struct epb_pool {
   int64_t launches = 0;
   int bytes_per_step = 0;
   bool started = false;  // a step, reset or rollout has been launched
+  bool imported = false;  // epb_state_import has loaded a blob (Go: with its configuration)
   // peer exchange (exchange.cuh):
   //   slot[D][world][x_slice] | data_flag[16] | ack_flag[16] | ctl | PeerView[D]
   char* x_base = nullptr;
@@ -195,9 +196,13 @@ struct epb_pool {
     ov.discount = static_cast<float*>(col(5));
     ov.step_type = static_cast<int32_t*>(col(6));
     ov.trunc = static_cast<uint8_t*>(col(7));
-    for (size_t k = 8; k < keys.size(); ++k) ov.env[k - 8] = col((int)k);
+    for (size_t k = 8; k < keys.size() && k < 13; ++k) ov.env[k - 8] = col((int)k);
     ov.t_stride_rows = N;
     return ov;
+  }
+  // env keys 5..9 of the slab at `base` (LaunchArgs::env_hi)
+  void slab_hi(char* base, void* (&hi)[kEnvKeys - 5]) const {
+    for (size_t k = 13; k < keys.size(); ++k) hi[k - 13] = base + keys[k].off;
   }
 };
 
@@ -543,6 +548,7 @@ int launch_batch(epb_pool* p, const void* d_action, const int32_t* d_ids, int n,
   p->started = true;
   LaunchArgs a = launch_args(p, stream);
   a.ov = p->slab_view(d_slab);
+  p->slab_hi(d_slab, a.env_hi);
   a.ov.wire = wire;
   a.action = d_action;
   a.env_ids = d_ids;
@@ -1064,10 +1070,11 @@ int epb_rollout_device(epb_pool* p, const void* d_actions, int T, void* const* d
   ov.discount = static_cast<float*>(d_cols[5]);
   ov.step_type = static_cast<int32_t*>(d_cols[6]);
   ov.trunc = static_cast<uint8_t*>(d_cols[7]);
-  for (size_t k = 8; k < p->keys.size(); ++k) ov.env[k - 8] = d_cols[k];
+  LaunchArgs a = launch_args(p, s);
+  for (size_t k = 8; k < p->keys.size(); ++k)
+    (k < 13 ? ov.env[k - 8] : a.env_hi[k - 13]) = d_cols[k];
   ov.t_stride_rows = p->N;
   p->started = true;
-  LaunchArgs a = launch_args(p, s);
   a.ov = ov;
   a.action = d_actions;
   a.n = p->N;
@@ -1620,6 +1627,7 @@ int epb_state_import(epb_pool* p, const void* host_src) {
   EPB_CUDA(guard.status);
   EPB_CUDA(cudaStreamSynchronize(p->stream));
   EPB_CUDA(cudaMemcpy(p->d_state_blob, host_src, (size_t)p->state_bytes, cudaMemcpyHostToDevice));
+  p->imported = true;
   if (p->fn.refill) {
     // a blob may carry a ring that is not full (a hand-edited RNG table wants its next resets
     // drawn from that table: rprod = rcons empties the ring): fill it now
@@ -1703,6 +1711,21 @@ int epb_minesweeper_config(epb_pool* p, const int32_t* mines100, const int32_t* 
   std::vector<uint32_t> words;
   if (const char* err = minesweeper_config(mines100, replay_boards3200, replay_rewards32,
                                            replay_done32, words))
+    return fail(EPB_ERR_INVALID, err);
+  DeviceGuard guard(p->cfg.device);
+  EPB_CUDA(guard.status);
+  EPB_CUDA(cudaMemcpy(p->sv.rstate, words.data(), 4 * words.size(), cudaMemcpyHostToDevice));
+  return EPB_OK;
+}
+int epb_go_config(epb_pool* p, double komi, int32_t max_terminal_steps) {
+  if (!p) return fail(EPB_ERR_INVALID, "null pool");
+  if (p->kind != EPB_GO_9X9 && p->kind != EPB_GO_13X13 && p->kind != EPB_GO_19X19)
+    return fail(EPB_ERR_INVALID, "not a Go pool");
+  if (p->started || p->imported)
+    return fail(EPB_ERR_STATE, "Go configuration must be set before the pool's first reset, "
+                               "step, rollout or state import");
+  std::vector<uint32_t> words;
+  if (const char* err = go_config(p->kind, komi, max_terminal_steps, words))
     return fail(EPB_ERR_INVALID, err);
   DeviceGuard guard(p->cfg.device);
   EPB_CUDA(guard.status);

@@ -61,10 +61,11 @@ struct OutView {
   float* discount;       // discount
   int32_t* step_type;    // step_type
   uint8_t* trunc;        // trunc
-  void* env[5];          // env-specific keys in declaration order
+  void* env[5];          // env-specific keys in declaration order (keys 5..9: LaunchArgs::env_hi)
   int32_t* wire;         // sharded pools: packed common columns for the peers (exchange.cuh)
   int64_t t_stride_rows; // rollout: rows between consecutive time steps (= N)
 };
+constexpr int kEnvKeys = 10;  // env keys of a kind: 5 in OutView::env, the rest in env_hi
 
 // ---------------------------------------------------------------------------------------
 // std::mt19937 on the device.
@@ -699,6 +700,8 @@ struct LaunchArgs {
   // step_kernel's prev_in_slab: set by run_chain alone, for the steps after the first of a chain
   // that writes p->d_slab (kernels that do not read it store every column anyway)
   int prev_in_slab;
+  // env keys 5..9 (Go's 10 columns): kept out of OutView, the parameter of every other kernel
+  void* env_hi[kEnvKeys - 5];
 };
 typedef cudaError_t (*launch_fn)(const LaunchArgs&);
 
@@ -799,7 +802,7 @@ struct KindLaunch {
 
 struct KindDesc {
   int kind;             // enum epb_kind
-  EnvKey keys[5];       // env columns after the 8 common ones (unused entries: name NULL)
+  EnvKey keys[kEnvKeys];  // env columns after the 8 common ones (unused entries: name NULL)
   EnvKey action;
   int NR, NI;           // real / int32 state words per env
   int config_words;     // int32 configuration words kept where rstate would be (0: rstate)
@@ -848,6 +851,7 @@ const KindDesc* toytext_kind(int kind);
 const KindDesc* jumanji_kind(int kind);
 const KindDesc* mujoco_kind(int kind);
 const KindDesc* pgx_kind(int kind);
+const KindDesc* go_kind(int kind);  // go.cu: the Go kinds, reached through pgx_kind
 
 // Jumanji configurations (jumanji.cu), packed into the config words its kernels read.  Either
 // argument may be NULL (not configured).  They return NULL, or the error when a cell is out of
@@ -857,5 +861,8 @@ const char* game2048_config(const int32_t* initial16, const int32_t* replay512,
 const char* minesweeper_config(const int32_t* mines100, const int32_t* replay_boards3200,
                                const float* replay_rewards32, const uint8_t* replay_done32,
                                std::vector<uint32_t>& words);
+// Go's komi and max_terminal_steps (go.cu), packed into its config words; NULL or the error.
+const char* go_config(int kind, double komi, int32_t max_terminal_steps,
+                      std::vector<uint32_t>& words);
 
 }  // namespace epb

@@ -42,7 +42,7 @@ namespace epb {
 constexpr int kMaxPeers = 16;
 constexpr int kMaxDepth = 8;
 
-constexpr int kMaxCols = 13;  // 8 common state keys + at most 5 env keys (OutView::env)
+constexpr int kMaxCols = 13;  // wire columns: reward, the env keys (Go: 10), the packed word
 
 struct ExchangeCtl {
   unsigned int blocks_done[kMaxDepth];       // last-block-done counter of the push into slot s

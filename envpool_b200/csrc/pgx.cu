@@ -671,6 +671,9 @@ const KindDesc kPgxKinds[] = {
      .action = kDiscreteAction, .NI = kStateWords<Othello>, .fp64_only = true,
      .launch = fixed_launch<Othello>, .players = Othello::kPlayers},
 };
-const KindDesc* pgx_kind(int kind) { return find_kind(kPgxKinds, kind); }
+const KindDesc* pgx_kind(int kind) {
+  if (const KindDesc* d = find_kind(kPgxKinds, kind)) return d;
+  return go_kind(kind);  // Go9x9, Go13x13, Go19x19 (go.cu)
+}
 
 }  // namespace epb

@@ -378,7 +378,49 @@ class SpecBase {
         action_cols.push_back(colb("action", 'i', {-1}, 0, actions - 1));
         break;
       }
+      case EPB_GO_19X19: {  // pgx/go.h GoEnvFns (every board size: go_kind picks the kernels)
+        const int size = go_size(), area = size * size;
+        state_cols.push_back(col("obs", 'b', {-1, size, size, 17}));
+        state_cols.push_back(colb("info:board", 'i', {size, size}, -1, 1));
+        state_cols.push_back(colb("info:current_player", 'i', {}, 0, 1));
+        state_cols.push_back(col("info:legal_action_mask", 'b', {area + 1}));
+        state_cols.push_back(colb("info:ko", 'i', {}, -1, area - 1));
+        state_cols.push_back(col("info:is_psk", 'b', {}));
+        state_cols.push_back(col("info:consecutive_pass_count", 'i', {}));
+        state_cols.push_back(col("info:black_area", 'i', {}));
+        state_cols.push_back(col("info:white_area", 'i', {}));
+        state_cols.push_back(colb("info:players.id", 'i', {-1}, 0, 1));
+        action_cols.push_back(colb("action", 'i', {-1}, 0, area));
+        break;
+      }
     }
+  }
+
+ public:
+  // Go's board_size after the checks of the accelerated path (ValueError outside it): the
+  // reference's boards 9, 13 and 19, history_length 8, max_terminal_steps in [0, 2 S^2] and the
+  // rules "pgx" / "tromp_taylor" ("chinese" masks repeated positions, which is not accelerated)
+  int go_size() const {
+    const int size = cfg<int>("board_size");
+    if (size != 9 && size != 13 && size != 19)
+      throw std::invalid_argument("Go: board_size " + std::to_string(size) +
+                                  " is not accelerated (9, 13 or 19)");
+    if (cfg<int>("history_length") != 8)
+      throw std::invalid_argument("Go: only history_length=8 is accelerated");
+    const int steps = cfg<int>("max_terminal_steps");
+    if (steps < 0 || steps > 2 * size * size)
+      throw std::invalid_argument("Go: max_terminal_steps must lie in [0, 2 * board_size^2]");
+    const std::string rules = cfg<std::string>("rules");
+    if (rules != "pgx" && rules != "tromp_taylor")
+      throw std::invalid_argument("Go: rules '" + rules +
+                                  "' are not accelerated ('pgx' or 'tromp_taylor')");
+    return size;
+  }
+  // the engine kind of the pool: Go's follows its board size
+  int engine_kind() const {
+    if (desc->kind != EPB_GO_19X19) return desc->kind;
+    const int size = go_size();
+    return size == 9 ? EPB_GO_9X9 : size == 13 ? EPB_GO_13X13 : EPB_GO_19X19;
   }
 };
 
@@ -497,7 +539,9 @@ class PoolBase {
     c.precision = prec == "f32" ? EPB_PREC_F32 : EPB_PREC_F64;
     c.env_id_offset = env_id_offset;
     h = std::make_shared<PoolHandle>();
-    check(epb_create(spec.desc->kind, &c, &h->p));
+    check(epb_create(spec.engine_kind(), &c, &h->p));
+    if (spec.desc->kind == EPB_GO_19X19)
+      check(epb_go_config(h->p, spec.cfg<double>("komi"), spec.cfg<int>("max_terminal_steps")));
     if (!spec.game2048_initial.empty() || !spec.game2048_replay.empty())
       check(epb_game2048_boards(
           h->p, spec.game2048_initial.empty() ? nullptr : spec.game2048_initial.data(),
@@ -759,7 +803,7 @@ PYBIND11_MODULE(EPB_MODULE_NAME, m) {
        });
   register_env<EPB_HALF_CHEETAH>(m, &desc_GymHalfCheetah);
 #elif defined(EPB_FAMILY_PGX)
-  // pgx/pgx.cc (TicTacToe, ConnectFour, Hex and Othello: the two-player board games on the
+  // pgx/pgx.cc (TicTacToe, ConnectFour, Hex, Othello and Go: the two-player board games on the
   // hot path)
   DESC_PLAYERS(TicTacToe, EPB_TIC_TAC_TOE, 2, S{"task"},
                { return py::make_tuple(std::string("tic_tac_toe")); });
@@ -772,6 +816,14 @@ PYBIND11_MODULE(EPB_MODULE_NAME, m) {
   register_env<EPB_CONNECT_FOUR>(m, &desc_ConnectFour);
   register_env<EPB_HEX>(m, &desc_Hex);
   register_env<EPB_OTHELLO>(m, &desc_Othello);
+  // pgx/go.h: one class for the three boards, as the reference's GoEnvSpec / GoEnvPool
+  DESC_PLAYERS(Go, EPB_GO_19X19, 2,
+               (S{"board_size", "komi", "history_length", "max_terminal_steps", "rules", "task"}),
+               {
+                 return py::make_tuple(19, 7.5, 8, 0, std::string("pgx"),
+                                       std::string("go_19x19"));
+               });
+  register_env<EPB_GO_19X19>(m, &desc_Go);
 #else
 #error "define one EPB_FAMILY_* macro"
 #endif

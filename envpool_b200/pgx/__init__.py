@@ -1,5 +1,6 @@
 """PGX family: binds the engine's pybind11 classes (`_TicTacToeEnvSpec` / `_TicTacToeEnvPool`,
-`_ConnectFourEnvSpec`, `_HexEnvSpec`, `_OthelloEnvSpec` and their pools, csrc/py_module.cc) to
+`_ConnectFourEnvSpec`, `_HexEnvSpec`, `_OthelloEnvSpec`, `_GoEnvSpec` and their pools,
+csrc/py_module.cc) to
 the Python adapters and exports `XxxEnvSpec`, `XxxDMEnvPool` and `XxxGymnasiumEnvPool` for each
 -- the names envpool/pgx/__init__.py exports for those games.  All are two-player pools: per-player columns
 (obs, reward, discount, info:players.env_id, info:players.id) hold two rows per env."""
@@ -13,8 +14,10 @@ ConnectFourEnvSpec, ConnectFourDMEnvPool, ConnectFourGymnasiumEnvPool = py_env(
 HexEnvSpec, HexDMEnvPool, HexGymnasiumEnvPool = py_env(_ext._HexEnvSpec, _ext._HexEnvPool)
 OthelloEnvSpec, OthelloDMEnvPool, OthelloGymnasiumEnvPool = py_env(
     _ext._OthelloEnvSpec, _ext._OthelloEnvPool)
+GoEnvSpec, GoDMEnvPool, GoGymnasiumEnvPool = py_env(_ext._GoEnvSpec, _ext._GoEnvPool)
 
 __all__ = ["TicTacToeEnvSpec", "TicTacToeDMEnvPool", "TicTacToeGymnasiumEnvPool",
            "ConnectFourEnvSpec", "ConnectFourDMEnvPool", "ConnectFourGymnasiumEnvPool",
            "HexEnvSpec", "HexDMEnvPool", "HexGymnasiumEnvPool",
-           "OthelloEnvSpec", "OthelloDMEnvPool", "OthelloGymnasiumEnvPool"]
+           "OthelloEnvSpec", "OthelloDMEnvPool", "OthelloGymnasiumEnvPool",
+           "GoEnvSpec", "GoDMEnvPool", "GoGymnasiumEnvPool"]

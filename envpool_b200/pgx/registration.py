@@ -1,5 +1,6 @@
 """PGX env registration (task ids, `task` and max_num_players as in envpool/pgx/registration.py;
-TicTacToe, ConnectFour, Hex and Othello are the accelerated PGX games)."""
+TicTacToe, ConnectFour, Hex, Othello and Go are the accelerated PGX games;
+ChineseGo*-v1 is not registered: its rules are not accelerated)."""
 from ..registration import register
 
 register(task_id="TicTacToe-v1", import_path="envpool_b200.pgx", spec_cls="TicTacToeEnvSpec",
@@ -14,3 +15,8 @@ register(task_id="Hex-v1", import_path="envpool_b200.pgx", spec_cls="HexEnvSpec"
 register(task_id="Othello-v1", import_path="envpool_b200.pgx", spec_cls="OthelloEnvSpec",
          dm_cls="OthelloDMEnvPool", gymnasium_cls="OthelloGymnasiumEnvPool", task="othello",
          max_num_players=2)
+for _size in (9, 13, 19):
+    register(task_id=f"Go{_size}x{_size}-v1", import_path="envpool_b200.pgx",
+             spec_cls="GoEnvSpec", dm_cls="GoDMEnvPool", gymnasium_cls="GoGymnasiumEnvPool",
+             board_size=_size, komi=7.5, history_length=8, max_terminal_steps=0, rules="pgx",
+             task=f"go_{_size}x{_size}", max_num_players=2)

@@ -34,6 +34,7 @@ _TASK_KWARGS = {
     "Blackjack": ("natural", "sab"),
     "HalfCheetah": ("frame_skip", "ctrl_cost_weight", "forward_reward_weight",
                     "reset_noise_scale", "post_constraint", "gymnasium_v5_render_camera"),
+    "Go": ("komi", "max_terminal_steps"),
 }
 # ... and of every multi-player kind: its registration's `task` and max_num_players
 _PLAYER_KWARGS = ("task", "max_num_players")
@@ -136,6 +137,11 @@ class ShardedPool:
                       reset_noise_scale=kwargs.get("reset_noise_scale", math.nan))
             if hc["frame_skip"] < 1:   # as make(): the reward divides by frame_skip * timestep
                 raise ValueError(f"HalfCheetah: frame_skip must be >= 1, got {hc['frame_skip']}")
+        go = {}
+        if engine_task == "Go":  # one engine kind per board size
+            engine_task = "Go{0}x{0}".format(kwargs["board_size"])
+            go = dict(komi=kwargs.get("komi", 7.5),
+                      max_terminal_steps=kwargs.get("max_terminal_steps", 0))
         self.group = group
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1
@@ -155,7 +161,7 @@ class ShardedPool:
         self.pool = _capi.CPool(engine_task, self.count, seed=seed,
                                 max_episode_steps=kwargs.get("max_episode_steps", -1),
                                 iopt=iopt, device=device, precision=precision,
-                                env_id_offset=self.offset, **hc)
+                                env_id_offset=self.offset, **hc, **go)
         self.stream = torch.cuda.ExternalStream(self.pool.stream, device=f"cuda:{device}")
         self._full = None
 
