@@ -37,6 +37,7 @@ CUDA_UNITS = {
     "mujoco.cu": [],
     "pgx.cu": [],
     "go.cu": [],
+    "chess.cu": [],
     "capi.cu": [],
 }
 PY_MODULES = {

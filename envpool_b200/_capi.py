@@ -38,6 +38,8 @@ ALL_KINDS = {**KINDS, **TWO_PLAYER_KINDS, **TWO_PLAYER_KINDS_2}
 # ... and Go, one kind per board size (tests/golden/pgx/go/); CPool takes its komi and
 # max_terminal_steps
 GO_KINDS = {"Go9x9": 18, "Go13x13": 19, "Go19x19": 20}
+# ... and the chess games, Chess and GardnerChess (tests/test_pgx_chess.py)
+CHESS_KINDS = {"Chess": 21, "GardnerChess": 22}
 DTYPES = {0: np.int32, 1: np.float32, 2: np.float64, 3: np.bool_}
 
 # every symbol include/envpool_b200.h declares (checked by tests/test_abi.py)
@@ -231,7 +233,7 @@ class CPool:
         cfg.forward_reward_weight = forward_reward_weight
         cfg.reset_noise_scale = reset_noise_scale
         h = ctypes.c_void_p()
-        kind = {**ALL_KINDS, **GO_KINDS}[task]
+        kind = {**ALL_KINDS, **GO_KINDS, **CHESS_KINDS}[task]
         _check(L.epb_create(kind, ctypes.byref(cfg), ctypes.byref(h)))
         self.h = h
         self.task = task

@@ -852,6 +852,7 @@ const KindDesc* jumanji_kind(int kind);
 const KindDesc* mujoco_kind(int kind);
 const KindDesc* pgx_kind(int kind);
 const KindDesc* go_kind(int kind);  // go.cu: the Go kinds, reached through pgx_kind
+const KindDesc* chess_kind(int kind);  // chess.cu: Chess and GardnerChess, through pgx_kind
 
 // Jumanji configurations (jumanji.cu), packed into the config words its kernels read.  Either
 // argument may be NULL (not configured).  They return NULL, or the error when a cell is out of

@@ -34,6 +34,7 @@
 #include <cstring>
 
 #include "common.cuh"
+#include "warp.cuh"
 
 namespace epb {
 
@@ -41,7 +42,6 @@ namespace {
 
 constexpr int kGoBlock = 128;  // 4 envs per CTA
 constexpr int kGoWarps = kGoBlock / 32;
-constexpr unsigned kFull = 0xffffffffu;
 
 template <int S>
 struct GoGeom {
@@ -77,11 +77,6 @@ __device__ __forceinline__ uint64_t warp_xor(uint64_t v) {
   for (int o = 16; o > 0; o >>= 1) v ^= __shfl_xor_sync(kFull, v, o);
   return v;
 }
-__device__ __forceinline__ int warp_sum(int v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-  return v;
-}
 __device__ __forceinline__ int sgn(int v) { return (v > 0) - (v < 0); }
 
 // Bitboards spread over the lanes, word k on lane k: shifts by 0 < k < 32 cells.
@@ -94,23 +89,6 @@ __device__ __forceinline__ uint32_t bb_shr(uint32_t w, int k, int lane) {
   uint32_t next = __shfl_down_sync(kFull, w, 1);
   if (lane == 31) next = 0u;
   return (w >> k) | (next << (32 - k));
-}
-
-// A warp writes n bytes at dst (any alignment), byte i = f(i): 4-byte stores in the middle.
-template <class F>
-__device__ __forceinline__ void warp_write_bytes(uint8_t* dst, int n, int lane, F f) {
-  int head = (int)((4u - ((uint32_t)(uintptr_t)dst & 3u)) & 3u);
-  head = head < n ? head : n;
-  if (lane < head) dst[lane] = f(lane);
-  const int words = (n - head) >> 2;
-  uint32_t* w = reinterpret_cast<uint32_t*>(dst + head);
-  for (int i = lane; i < words; i += 32) {
-    const int b = head + 4 * i;
-    w[i] = (uint32_t)f(b) | ((uint32_t)f(b + 1) << 8) | ((uint32_t)f(b + 2) << 16) |
-           ((uint32_t)f(b + 3) << 24);
-  }
-  const int tail0 = head + 4 * words;
-  if (tail0 + lane < n) dst[tail0 + lane] = f(tail0 + lane);
 }
 
 template <int S>

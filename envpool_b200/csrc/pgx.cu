@@ -673,7 +673,8 @@ const KindDesc kPgxKinds[] = {
 };
 const KindDesc* pgx_kind(int kind) {
   if (const KindDesc* d = find_kind(kPgxKinds, kind)) return d;
-  return go_kind(kind);  // Go9x9, Go13x13, Go19x19 (go.cu)
+  if (const KindDesc* d = go_kind(kind)) return d;  // Go9x9, Go13x13, Go19x19 (go.cu)
+  return chess_kind(kind);                           // Chess, GardnerChess (chess.cu)
 }
 
 }  // namespace epb

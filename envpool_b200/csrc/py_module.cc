@@ -378,6 +378,23 @@ class SpecBase {
         action_cols.push_back(colb("action", 'i', {-1}, 0, actions - 1));
         break;
       }
+      case EPB_CHESS:           // pgx/chess_games.h ChessEnvFns
+      case EPB_GARDNER_CHESS: {  // pgx/chess_games.h GardnerChessEnvFns
+        const bool chess = desc->kind == EPB_CHESS;
+        const int size = chess ? 8 : 5, actions = chess ? 4672 : 1225;
+        state_cols.push_back(col("obs", 'f', {-1, size, size, chess ? 119 : 115}));
+        state_cols.push_back(col("info:board", 'i', {size, size}));
+        if (chess) state_cols.push_back(col("info:castling_rights", 'b', {2, 2}));
+        state_cols.push_back(colb("info:current_player", 'i', {}, 0, 1));
+        if (chess) state_cols.push_back(colb("info:en_passant", 'i', {}, -1, 63));
+        state_cols.push_back(col("info:fullmove_count", 'i', {}));
+        state_cols.push_back(col("info:halfmove_count", 'i', {}));
+        state_cols.push_back(col("info:legal_action_mask", 'b', {actions}));
+        state_cols.push_back(colb("info:players.id", 'i', {-1}, 0, 1));
+        state_cols.push_back(colb("info:turn", 'i', {}, 0, 1));
+        action_cols.push_back(colb("action", 'i', {-1}, 0, actions - 1));
+        break;
+      }
       case EPB_GO_19X19: {  // pgx/go.h GoEnvFns (every board size: go_kind picks the kernels)
         const int size = go_size(), area = size * size;
         state_cols.push_back(col("obs", 'b', {-1, size, size, 17}));
@@ -803,7 +820,8 @@ PYBIND11_MODULE(EPB_MODULE_NAME, m) {
        });
   register_env<EPB_HALF_CHEETAH>(m, &desc_GymHalfCheetah);
 #elif defined(EPB_FAMILY_PGX)
-  // pgx/pgx.cc (TicTacToe, ConnectFour, Hex, Othello and Go: the two-player board games on the
+  // pgx/pgx.cc (TicTacToe, ConnectFour, Hex, Othello, Go and the chess games: the two-player board
+  // games on the
   // hot path)
   DESC_PLAYERS(TicTacToe, EPB_TIC_TAC_TOE, 2, S{"task"},
                { return py::make_tuple(std::string("tic_tac_toe")); });
@@ -824,6 +842,12 @@ PYBIND11_MODULE(EPB_MODULE_NAME, m) {
                                        std::string("go_19x19"));
                });
   register_env<EPB_GO_19X19>(m, &desc_Go);
+  // pgx/chess_games.h
+  DESC_PLAYERS(Chess, EPB_CHESS, 2, S{"task"}, { return py::make_tuple(std::string("chess")); });
+  DESC_PLAYERS(GardnerChess, EPB_GARDNER_CHESS, 2, S{"task"},
+               { return py::make_tuple(std::string("gardner_chess")); });
+  register_env<EPB_CHESS>(m, &desc_Chess);
+  register_env<EPB_GARDNER_CHESS>(m, &desc_GardnerChess);
 #else
 #error "define one EPB_FAMILY_* macro"
 #endif

@@ -1,5 +1,5 @@
 """PGX env registration (task ids, `task` and max_num_players as in envpool/pgx/registration.py;
-TicTacToe, ConnectFour, Hex, Othello and Go are the accelerated PGX games;
+TicTacToe, ConnectFour, Hex, Othello, Go, Chess and GardnerChess are the accelerated PGX games;
 ChineseGo*-v1 is not registered: its rules are not accelerated)."""
 from ..registration import register
 
@@ -20,3 +20,9 @@ for _size in (9, 13, 19):
              spec_cls="GoEnvSpec", dm_cls="GoDMEnvPool", gymnasium_cls="GoGymnasiumEnvPool",
              board_size=_size, komi=7.5, history_length=8, max_terminal_steps=0, rules="pgx",
              task=f"go_{_size}x{_size}", max_num_players=2)
+register(task_id="Chess-v1", import_path="envpool_b200.pgx", spec_cls="ChessEnvSpec",
+         dm_cls="ChessDMEnvPool", gymnasium_cls="ChessGymnasiumEnvPool", task="chess",
+         max_num_players=2)
+register(task_id="GardnerChess-v1", import_path="envpool_b200.pgx", spec_cls="GardnerChessEnvSpec",
+         dm_cls="GardnerChessDMEnvPool", gymnasium_cls="GardnerChessGymnasiumEnvPool",
+         task="gardner_chess", max_num_players=2)
